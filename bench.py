@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py -- headline benchmark of the B200 block-cost path (contract: see DESIGN.md section "Measurement").
+"""bench.py -- headline benchmark of the H100 block-cost path (contract: see DESIGN.md section "Measurement").
 
 Workload `2160p10_fullsearch_me_rdo` (BASELINE.json: candidate-blocks/s (SAD+SATD+DCT-quant) on 2160p10):
 one 3840x2160 10-bit luma picture against one reference picture; for every block of the quad-tree depths
@@ -14,6 +14,8 @@ run is then seconds, not milliseconds); units = candidate-blocks = SAD candidate
   e2e   : same step through the host-buffer C ABI (pictures + block lists uploaded, costs / vectors / levels downloaded
           for every picture), pinned host memory
   --impl reference : the reference's own AVX2 path (oracle/_ref, else the oracle port) on the host cores, bounded sample
+  --dump-outputs DIR : after the timed steps, the per-block results of the last timed picture (search vectors and costs, SATD pattern costs, levels,
+          absSum, last position, RDOQ flag) for a fixed seeded sample of blocks per size, as DIR/<name>_<size>.npy (float64 / float32)
 
 N > 1 (torchrun): CTU-row bands (vvenc_b200.bands.split_ctu_rows) of ONE picture that is N times taller (weak scaling: 3840 x 2160*N, replicated on
 every rank); every rank runs the kernels on its band; one NCCL all-gather of the per-block result tables per picture (bands.BandGather); after the
@@ -32,9 +34,10 @@ SIZES = (8, 16, 32, 64)
 SEARCH_RANGE = 32
 QP = 32
 LAMBDA = 57.9          # ~ 0.57 * 2^((QP-12)/3), the encoder's lambda scale at QP 32
-N_PICTURE_SETS = 4     # rotated between pictures: 4 x (org+ref) = 4 x 36.6 MB planes + outputs > 126 MB L2
+N_PICTURE_SETS = 4     # rotated between pictures: 4 x (org+ref) = 4 x 36.6 MB planes + outputs > 50 MB L2
 PICTURES_PER_STEP = 40
 CTU = 128
+DUMP_BLOCKS = 1024     # --dump-outputs: blocks sampled per size (64x64 levels of 1024 blocks = 16 MB as float32)
 
 
 def refine_pattern():
@@ -149,29 +152,7 @@ def measured_peaks():
             return float(d['hbm_gbs']), 'measured (MEASURED_PEAKS.json)'
         except Exception:
             pass
-    return 6650.0, 'fallback (B200_PROFILING.md)'
-
-
-def ncu_dram_traffic(kernel_substr, profiles=('profiles/r02p_ncu_step_kernels.txt', 'profiles/r02_ncu_step_kernels.txt', 'profiles/r01_v8_ncu_step_kernels.txt')):
-    """dram__bytes_read.sum + dram__bytes_write.sum (bytes per launch) of the first capture whose kernel name contains `kernel_substr`, from the committed
-    `ncu --set full` summaries; (None, None) when no file holds the kernel"""
-    unit = {'byte': 1.0, 'Kbyte': 1e3, 'Mbyte': 1e6, 'Gbyte': 1e9}
-    for profile in profiles:
-        try:
-            for blk in open(os.path.join(ROOT, profile)).read().split('-' * 100):
-                name = [l for l in blk.split('\n') if l.startswith('Kernel Name')]
-                if not name or kernel_substr not in name[0]:
-                    continue
-                tot = 0.0; seen = 0
-                for l in blk.split('\n'):
-                    if l.startswith('dram__bytes_read.sum') or l.startswith('dram__bytes_write.sum'):
-                        f = l.split()
-                        tot += float(f[1].replace(',', '')) * unit[f[2]]; seen += 1
-                if seen == 2:
-                    return tot, profile
-        except Exception:
-            continue
-    return None, None
+    return 3350.0, 'data sheet (H100 SXM HBM3)'
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -487,6 +468,28 @@ class Job:
         return {n: (self.d_best[n][:self.counts[n] * 16].clone(), self.d_satd[n].clone(), self.d_sum[n].clone(), self.d_last[n].clone(), self.d_q[n].clone()) for n in SIZES}
 
 
+def dump_outputs(out_dir, job, env):
+    """what the timed path hands its caller for the last picture it ran: per size, the same seeded sample of blocks of every result table"""
+    V, KP = env['V'], env['KP']
+    os.makedirs(out_dir, exist_ok=True)
+    rs = np.random.RandomState(0)
+    for n in SIZES:
+        nb = job.counts[n]
+        if nb == 0:
+            continue
+        sel = np.sort(rs.choice(nb, min(nb, DUMP_BLOCKS), replace=False))
+        best = np.frombuffer(job.d_best[n][:nb * 16].cpu().numpy().tobytes(), dtype=V.BEST_DT)[sel]
+        arrays = {'block_index': sel.astype(np.float64),
+                  'best_mv_sad_cost': np.stack([best['dx'], best['dy'], best['sad'], best['cost']], axis=1).astype(np.float64),
+                  'satd': job.d_satd[n][:nb * KP].cpu().numpy().reshape(nb, KP)[sel].astype(np.float64),
+                  'levels': job.d_q[n][:nb * n * n].cpu().numpy().reshape(nb, n, n)[sel].astype(np.float32),
+                  'abs_sum': job.d_sum[n][:nb].cpu().numpy()[sel].astype(np.float64),
+                  'last_pos': job.d_last[n][:nb].cpu().numpy()[sel].astype(np.float64),
+                  'need_rdoq': job.d_nr[n][:nb].cpu().numpy()[sel].astype(np.float32)}
+        for name, a in arrays.items():
+            np.save(os.path.join(out_dir, '%s_%d.npy' % (name, n)), a)
+
+
 def sharded_parity(env, jobs_all_bands, gather, po, pr, own_job):
     """rank 0: every band recomputed on this GPU alone must equal what the band's owner sent through the all-gather, bit for bit"""
     torch, eng = env['torch'], env['eng']
@@ -612,6 +615,7 @@ def main():
     ap.add_argument('--skip-cpu', action='store_true', help='profiling runs: no CPU baseline leg')
     ap.add_argument('--skip-extras', action='store_true', help='profiling runs: no per-kernel rows')
     ap.add_argument('--strong', action='store_true', help='also run the 4320p strong-scaling case at N = 1 (always run for N > 1)')
+    ap.add_argument('--dump-outputs', metavar='DIR', help='write the results of the last timed picture (seeded sample of blocks) as DIR/*.npy')
     args = ap.parse_args()
     rank = int(os.environ.get('RANK', '0')); world = int(os.environ.get('WORLD_SIZE', '1')); local = int(os.environ.get('LOCAL_RANK', '0'))
     PPS = max(1, args.pictures_per_step)
@@ -746,6 +750,8 @@ def main():
         sampler.start()
     ms_total, launches = timed(step_resident, args.steps, max(3, args.warmup))
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, job, env)
     ms_step = ms_total / args.steps
     ms_picture = ms_step / PPS
     value = units_picture_all * PPS / (ms_step * 1e-3)
@@ -817,28 +823,24 @@ def main():
             t_search += kt[n]['sad_search_ms']
             pel_diffs += nb * nx * nx * n * n
         # issue ceiling of the packed-SAD instruction pair: the alu pipe (VIMNMX.S16x2) and the fma pipe (IDP.2A) each take one warp instruction every second
-        # cycle per scheduler (B300_MICROARCH.md "fma vs alu split"), so one min + one dot product per pel PAIR = 1 pel difference per lane and cycle at best
-        sm_mhz = (clocks or {}).get('sm_max_mhz') or 1965.0
-        issue_peak = 148 * 4 * 32 * sm_mhz * 1e6
-        ctas, iters = 148 * 8, 4096
+        # cycle per scheduler, so one min + one dot product per pel PAIR = 1 pel difference per lane and cycle at best
+        sms = torch.cuda.get_device_properties(local).multi_processor_count
+        sm_mhz = (clocks or {}).get('sm_max_mhz') or 1980.0
+        issue_peak = sms * 4 * 32 * sm_mhz * 1e6
+        ctas, iters = sms * 8, 4096
         t_probe = time_launch(lambda: chk(lib.vvb_alu_probe_dev(eng.h, ctas, iters, 1)), reps=5)
         alu_probe = ctas * 256 * iters * 16 / (t_probe * 1e-3)
         n0 = SIZES[0]; nb0 = len(blocks_np[n0])
         pyr_bytes = nb0 * (2 * n0 * n0 + 2 * (n0 + 2 * SEARCH_RANGE) ** 2 + 16)            # SURVEY 8d W2: compulsory bytes per block, base level (the only pel pass)
         pyr_pel = nb0 * nx * nx * n0 * n0                                                     # pel differences actually evaluated by the pyramid
         ach_alu = pyr_pel / (t_pyr * 1e-3)
-        traffic, traffic_src = ncu_dram_traffic('sad_pyramid8_kernel<4>')
-        if traffic is None:
-            traffic, traffic_src = ncu_dram_traffic('sad_search_kernel<1, 1, 1>')
-            traffic_src = (traffic_src or '') + ' (round-1 kernel; the in-CTA pyramid has no capture in this checkout yet)'
         roofline = {'kernel': 'sad_pyramid8_kernel<4> (vvb_sad_search_pyramid_dev: one CTA per 64x64 root, all four levels on the SM)', 'bound': 'alu',
                     'achieved': ach_alu / 1e12, 'peak': issue_peak / 1e12, 'unit': 'Tpel-diff/s', 'frac': ach_alu / issue_peak,
-                    'peak_source': 'issue ceiling 148 SM x 4 schedulers x 32 lanes x %.0f MHz: one VIMNMX.S16x2 (alu pipe) + one IDP.2A (fma pipe) per pel pair, each pipe '
-                                   'accepting a warp instruction every 2nd cycle' % sm_mhz,
+                    'peak_source': 'issue ceiling %d SM x 4 schedulers x 32 lanes x %.0f MHz: one VIMNMX.S16x2 (alu pipe) + one IDP.2A (fma pipe) per pel pair, each pipe '
+                                   'accepting a warp instruction every 2nd cycle' % (sms, sm_mhz),
                     'probe': {'achieved_by_register_only_probe': alu_probe / 1e12, 'frac_of_probe': ach_alu / alu_probe,
                               'note': 'alu_probe_kernel: the same instruction pair on register operands, measured in this run'},
                     'ms_per_launch': t_pyr, 'share_of_step': t_pyr / ms_picture,
-                    'traffic': traffic, 'traffic_source': 'dram__bytes_read.sum + dram__bytes_write.sum per launch, ' + str(traffic_src),
                     'hbm': {'achieved': pyr_bytes / (t_pyr * 1e-3) / 1e9, 'peak': hbm_peak, 'unit': 'GB/s', 'frac': pyr_bytes / (t_pyr * 1e-3) / 1e9 / hbm_peak,
                             'peak_source': peak_src, 'bytes': 'compulsory 2N^2 + 2(N+2R)^2 + 16 per 8x8 block (SURVEY 8d W2): small by construction, every reference '
                                                               'pel is re-used up to 4225x from shared memory'},
@@ -1009,7 +1011,7 @@ def main():
                 byt = nb * Kt * (2 * n * n + 2 * n * n / Kt + 8)
                 dia[str(n)] = {'ms': t, 'cand_per_s': nb * Kt / (t * 1e-3), 'GBps_w1_formula': byt / (t * 1e-3) / 1e9, 'frac_hbm_w1_formula': byt / (t * 1e-3) / 1e9 / hbm_peak}
             extra['diamond_set_sad'] = {'points': Kt, 'range': 64, 'note': 'candidates overlap in the L2-resident reference plane: the W1 byte formula counts every candidate block '
-                                        'as fresh bytes, so fractions above 1.0 mean L2 hits, not missing work (DRAM traffic in profiles/)', **dia}
+                                        'as fresh bytes, so fractions above 1.0 mean L2 hits, not missing work', **dia}
         except Exception as ex:
             extra['diamond_set_sad'] = {'error': str(ex)}
         # fast RDOQ (SURVEY 8f-4, QuantRDOQ2::xRateDistOptQuantFast, what Quant::m_RDOQ == 2 of the presets faster / fast runs): one TU per thread, bound by the serial
@@ -1030,14 +1032,14 @@ def main():
                 par = eng.tu_par(n, n, 0, 0, BITDEPTH, QP, sign_hiding=True); rqp = VL.vvb_rdoq_par(57.3, 8, 0)
                 row = {'tus': int(cnt)}
                 for mult in (1, 16):
-                    d_c = torch.from_numpy(coef).cuda().repeat(mult, 1, 1); d_q = torch.zeros((cnt * mult, n, n), dtype=torch.int16, device='cuda')
+                    d_c = torch.from_numpy(coef).cuda().repeat(mult, 1, 1); d_rq = torch.zeros((cnt * mult, n, n), dtype=torch.int16, device='cuda')
                     d_s = torch.zeros(cnt * mult, dtype=torch.int32, device='cuda'); d_l = torch.zeros(cnt * mult, dtype=torch.int32, device='cuda')
                     t = time_launch(lambda: chk(lib.vvb_rdoq_dev(eng.h, ctypes.byref(par), ctypes.byref(rqp), ctypes.byref(rates), P_(d_c.data_ptr()), None, cnt * mult,
-                                                                 P_(d_q.data_ptr()), P_(d_s.data_ptr()), P_(d_l.data_ptr()))), reps=3)
+                                                                 P_(d_rq.data_ptr()), P_(d_s.data_ptr()), P_(d_l.data_ptr()))), reps=3)
                     row['ms_per_picture' if mult == 1 else 'ms_per_picture_at_16_pictures'] = t / mult
                     if mult == 1:
-                        q_dev = d_q.cpu().numpy(); l_dev = d_l.cpu().numpy()
-                    del d_c, d_q, d_s, d_l
+                        q_dev = d_rq.cpu().numpy(); l_dev = d_l.cpu().numpy()
+                    del d_c, d_rq, d_s, d_l
                 qq = np.zeros((cnt, n, n), dtype=np.int16); ss = np.zeros(cnt, dtype=np.int32); ll = np.zeros(cnt, dtype=np.int32)
                 t0 = time.perf_counter()
                 dq_oracle().orc_rdoq(n, n, BITDEPTH, QP, 0, 0, 0, 1, 57.3, 8, P_np(rates_flat), P_np(coef), cnt, P_np(qq), P_np(ss), P_np(ll))

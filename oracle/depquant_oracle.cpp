@@ -5,7 +5,7 @@
  * CommonLib/DepQuant.cpp it follows) and the table / constant set-up is depquant_host.h; this file compiles both with g++ so that
  *   - tests/test_oracle_vs_reference.py can pin the restatement against the reference's own DepQuant::quant (oracle/_ref probe, scalar and AVX2 members) and
  *     against the golden vectors the reference generated (tests/golden/depquant_*.npz), here, without a GPU;
- *   - the GPU tests compare the device kernel (the same text compiled by nvcc for sm_100a) with this build on the same inputs.
+ *   - the GPU tests compare the device kernel (the same text compiled by nvcc for sm_90a) with this build on the same inputs.
  * The product library never loads this file.
  */
 #include "../vvenc_b200/csrc/depquant_core.h"

@@ -5,7 +5,7 @@
  * CommonLib/QuantRDOQ2.cpp / ContextModelling.h it follows) and the constant set-up is rdoq_host.h; this file compiles both with g++ so that
  *   - tests/test_oracle_vs_reference.py can pin the restatement against the reference's own QuantRDOQ2::xRateDistOptQuant (oracle/_ref probe) and against the
  *     golden vectors the reference generated (tests/golden/golden_v6_rdoq.npz), here, without a GPU;
- *   - the GPU tests compare the device kernel (the same text compiled by nvcc for sm_100a) with this build on the same inputs.
+ *   - the GPU tests compare the device kernel (the same text compiled by nvcc for sm_90a) with this build on the same inputs.
  * The product library never loads this file.
  */
 #include "../vvenc_b200/csrc/rdoq_core.h"

@@ -482,7 +482,7 @@ def test_gpu_lfnst_inverse_and_roundtrip_vs_oracle(gpu):
 
 
 def test_gpu_raw_byte_tensor_engine_vs_cuda_core_engine_and_oracle(gpu):
-    """vvb_set_tensor_transform(3): the tcgen05 engine whose MMA operands are the raw bytes of the residual / the stage-1 values (trquant_tc2_kernels.cuh), square TUs
+    """vvb_set_tensor_transform(3): the wgmma engine whose MMA operands are the raw bytes of the residual / the stage-1 values (trquant_tc2_kernels.cuh), square TUs
     8..64: compact pools and residuals formed from planes (every pel alignment of org and pred), all transform pairs, 8/10/12 bit, tails that do not fill a tile,
     int16 extremes (the full input domain is exact), with and without the coefficient output -- levels, coefficients, absSum, lastPos and the RDOQ flag equal the
     CUDA-core engine on everything and the oracle on a sample"""
@@ -545,13 +545,13 @@ def _tc2_planes(rs, W, H, m, bd=10):
 
 
 def test_gpu_inverse_tensor_engine_vs_cuda_core_engine(gpu):
-    """vvb_set_tensor_transform(3) also routes vvb_inv_trquant and the second half of vvb_tu_roundtrip of square 8 / 16 / 32 TUs through the tcgen05 inverse engine
+    """vvb_set_tensor_transform(3) also routes vvb_inv_trquant and the second half of vvb_tu_roundtrip of square 8 / 16 / 32 / 64 TUs through the wgmma inverse engine
     (itrquant_tc_kernels.cuh: dequantised coefficients and first-pass outputs as raw int16 bytes): residuals, reconstructions and the three distortions equal the
     CUDA-core engine for every transform pair, 8 / 10 / 12 bit, plain and DepQuant dequantiser, levels up to the int16 extremes, tails that do not fill a tile, and
     resident-plane addressing with any prediction displacement"""
     rs = np.random.RandomState(4004)
     try:
-        for (N, pairs) in ((8, ((0, 0), (2, 2), (1, 2))), (16, ((0, 0), (2, 1))), (32, ((0, 0), (1, 2), (2, 2)))):
+        for (N, pairs) in ((8, ((0, 0), (2, 2), (1, 2))), (16, ((0, 0), (2, 1))), (32, ((0, 0), (1, 2), (2, 2))), (64, ((0, 0),))):
             for (th, tv) in pairs:
                 for bd in (8, 10, 12):
                     for dq in (0, 1):
@@ -592,3 +592,34 @@ def test_gpu_inverse_tensor_engine_vs_cuda_core_engine(gpu):
             assert np.array_equal(a['q'], b['q']) and np.array_equal(a['reco'], b['reco']) and np.array_equal(a['res'], b['res']) and np.array_equal(a['need_rdoq'], b['need_rdoq']), N
     finally:
         gpu.eng.set_tensor_transform(3)
+
+
+def test_gpu_tensor_engines_run_at_every_square_size(gpu):
+    """with vvb_set_tensor_transform(3) the raw-byte wgmma kernels themselves run for square 8 / 16 / 32 / 64 TUs: fwd_trquant_tc2_kernel for
+    vvb_fwd_trquant, inv_trquant_tc_kernel for vvb_inv_trquant, both for vvb_tu_roundtrip -- the kernel names in a torch.profiler trace of each call"""
+    import torch
+    from torch.profiler import profile, ProfilerActivity
+    rs = np.random.RandomState(77)
+    gpu.eng.set_tensor_transform(3)
+
+    def kernels(fn):
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            fn()
+            torch.cuda.synchronize()
+        return [e.name for e in prof.events()]
+
+    def count(names, kernel, N):
+        return sum(1 for e in names if '%s<%d,' % (kernel, N) in e or '%sILi%dE' % (kernel, N) in e)
+
+    for N in (8, 16, 32, 64):
+        par = gpu.eng.tu_par(N, N, 0, 0, 10, 30, False, False)
+        resi = rs.randint(-300, 301, size=(5, N, N)).astype(np.int16)
+        org = rs.randint(0, 1024, size=(5, N, N)).astype(np.int16)
+        pred = np.clip(org + rs.randint(-60, 61, size=org.shape), 0, 1023).astype(np.int16)
+        q = gpu.eng.fwd_trquant(par, resi)['q']
+        fwd = kernels(lambda: gpu.eng.fwd_trquant(par, resi))
+        inv = kernels(lambda: gpu.eng.inv_trquant(par, q))
+        rt = kernels(lambda: gpu.eng.tu_roundtrip(par, org, pred))
+        assert count(fwd, 'fwd_trquant_tc2_kernel', N) == 1, (N, sorted(set(fwd)))
+        assert count(inv, 'inv_trquant_tc_kernel', N) == 1, (N, sorted(set(inv)))
+        assert count(rt, 'fwd_trquant_tc2_kernel', N) == 1 and count(rt, 'inv_trquant_tc_kernel', N) == 1, (N, sorted(set(rt)))

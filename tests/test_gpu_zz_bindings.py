@@ -2,7 +2,7 @@
 libvvenc_b200.so and run next to the reference's own member functions -- the comparison tests/test_integration_host.py makes on the CPU with the oracle-backed
 mock, with the kernels answering instead.  Runs in a process of its own (the probe binds one library per process) and last in the suite.
 
-First ran on hardware at the end of round 1 (XPASS in GPUTEST_r01.json); the xfail guard is gone since."""
+First ran on hardware at the end of round 1; the xfail guard is gone since."""
 import json
 import os
 import subprocess

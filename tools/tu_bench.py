@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Component timing of the TU kernels on pools larger than L2: forward (tcgen05 / IDP.2A), inverse, fused round trip.
+"""Component timing of the TU kernels on pools larger than L2: forward (wgmma / IDP.2A), inverse, fused round trip.
 usage: python tools/tu_bench.py [noise_amp [WxH ...]]   (GPU box)"""
 import ctypes, sys, os
 import numpy as np, torch

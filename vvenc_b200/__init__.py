@@ -1,4 +1,4 @@
-"""vvenc_b200 -- B200-native (sm_100a) implementation of VVenC's block-cost hot path:
+"""vvenc_b200 -- H100-native (sm_90a) implementation of VVenC's block-cost hot path:
 SAD / SATD / SSE distortion kernels, fixed-pattern and full-search motion sweeps, forward DCT-II/DST-VII/DCT-VIII +
 quantisation, MCTF block matching and the affine gradient helpers, behind a C ABI (include/vvenc_b200.h).
 

@@ -180,7 +180,7 @@ def load():
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise RuntimeError('vvenc_b200: %s is missing -- run `python -c "import __graft_entry__ as g; g.build()"` '
-                               '(nvcc, sm_100a); there is no CPU fallback' % LIB_PATH)
+                               '(nvcc, sm_90a); there is no CPU fallback' % LIB_PATH)
         lib = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in SYMBOLS.items():
             f = getattr(lib, name)          # AttributeError if the export is missing

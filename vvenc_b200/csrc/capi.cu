@@ -269,6 +269,10 @@ int vvb_create( vvb_ctx** out, int device )
                           cudaFuncSetAttribute( fwd_trquant_tc2_kernel<Nv, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, Tc2Shape<Nv>::SMEM );
   VVB_TC2_ATTR( 8 ) VVB_TC2_ATTR( 16 ) VVB_TC2_ATTR( 32 ) VVB_TC2_ATTR( 64 )
 #undef VVB_TC2_ATTR
+#define VVB_ITC_ATTR( Nv ) cudaFuncSetAttribute( inv_trquant_tc_kernel<Nv, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, ItcShape<Nv>::SMEM ); \
+                          cudaFuncSetAttribute( inv_trquant_tc_kernel<Nv, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ItcShape<Nv>::SMEM );
+  VVB_ITC_ATTR( 8 ) VVB_ITC_ATTR( 16 ) VVB_ITC_ATTR( 32 ) VVB_ITC_ATTR( 64 )
+#undef VVB_ITC_ATTR
   cudaFuncSetAttribute( fwd_trquant_tc_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024 );
   cudaFuncSetAttribute( fwd_trquant_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024 );
   cudaFuncSetAttribute( fwd_trquant_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024 );
@@ -331,7 +335,7 @@ int vvb_set_pyramid_engine( vvb_ctx* ctx, int engine )
   return VVB_OK;
 }
 
-// selects the transform engine for square 16/32/64 TUs: 1 = tcgen05 tensor cores (default), 0 = IDP.2A CUDA-core kernel
+// selects the transform engine (include/vvenc_b200.h): 3 = raw-byte wgmma engine (default), 1 / 2 = byte-plane wgmma engine, 0 = IDP.2A CUDA-core kernels
 int vvb_set_tensor_transform( vvb_ctx* ctx, int enable )
 {
   if( !ctx ) return VVB_ERR_ARG;
@@ -1194,15 +1198,15 @@ static int tc2Launch( vvb_ctx* ctx, const TuPar& p, const int16_t* dResi, int or
     ctx->tc2Image[key] = d;
   }
   const uint4* dImg = (const uint4*) ctx->tc2Image[key];
-  const char* envC = getenv( "VVB_TC2_CTAS" ); const char* envS = getenv( "VVB_TC2_STREAM" );     // tuning knobs: CTAs per SM; bit 0 cp.async streaming, bit 1 single-thread wait
-  const int capC = envC ? atoi( envC ) : 0, streamOn = envS ? atoi( envS ) : 3;
+  const char* envC = getenv( "VVB_TC2_CTAS" ); const char* envS = getenv( "VVB_TC2_STREAM" );     // tuning knobs: CTAs per SM; bit 0 cp.async streaming
+  const int capC = envC ? atoi( envC ) : 0, streamOn = envS ? atoi( envS ) : 1;
 #define VVB_TC2_CALL( Nv ) { using S = Tc2Shape<Nv>; const int tiles = ( n + S::TPT - 1 ) / S::TPT; \
     static int perSm[3] = { 0, 0, 0 }; const int mode = dBlocks ? 1 : dResi2 ? 2 : 0; int& ps = perSm[mode]; \
     if( !ps ) { cudaFuncAttributes fa = {}; \
                 if( mode == 1 ) cudaFuncGetAttributes( &fa, fwd_trquant_tc2_kernel<Nv, 1> ); else if( mode == 2 ) cudaFuncGetAttributes( &fa, fwd_trquant_tc2_kernel<Nv, 2> ); \
                 else cudaFuncGetAttributes( &fa, fwd_trquant_tc2_kernel<Nv, 0> ); \
                 const int regs = std::max( fa.numRegs, 32 ); \
-                ps = std::min( std::min( 65536 / ( regs * 128 ), ( 227 * 1024 ) / ( (int) S::SMEM + (int) fa.sharedSizeBytes + 1024 ) ), 512 / S::TMEM_COLS ); ps = std::max( std::min( ps, Nv == 8 ? 6 : 8 ), 1 ); } \
+                ps = std::min( 65536 / ( regs * 128 ), ( 227 * 1024 ) / ( (int) S::SMEM + (int) fa.sharedSizeBytes + 1024 ) ); ps = std::max( std::min( ps, Nv == 8 ? 6 : 8 ), 1 ); } \
     const int grid = std::min( tiles, ctx->numSMs * ( capC > 0 ? std::min( capC, ps ) : ps ) ); \
     if( mode == 1 )      fwd_trquant_tc2_kernel<Nv, 1><<<grid, 128, S::SMEM, ctx->stream>>>( p, dImg, streamOn, ctx->d_scan, nullptr, nullptr, po, pp, dBlocks, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq ); \
     else if( mode == 2 ) fwd_trquant_tc2_kernel<Nv, 2><<<grid, 128, S::SMEM, ctx->stream>>>( p, dImg, streamOn, ctx->d_scan, dResi, dResi2, po, pp, nullptr, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq ); \
@@ -1237,7 +1241,7 @@ static int itcLaunch( vvb_ctx* ctx, const TuPar& p, const int16_t* dQ, int n, in
   }
   const uint4* dImg = (const uint4*) ctx->itcImage[key];
   const Plane po = dBlocks ? ctx->planes.p[orgPlane] : Plane{}, pp = dBlocks ? ctx->planes.p[predPlane] : Plane{};
-#define VVB_ITC_CALL( Nv ) { using S = ItcShape<Nv>; const int tiles = ( n + S::TPT - 1 ) / S::TPT; const int grid = std::min( tiles, ctx->numSMs * std::min( 6, 512 / S::TMEM_COLS ) ); \
+#define VVB_ITC_CALL( Nv ) { using S = ItcShape<Nv>; const int tiles = ( n + S::TPT - 1 ) / S::TPT; const int grid = std::min( tiles, ctx->numSMs * std::min( 6, ( 227 * 1024 ) / ( S::SMEM + 1024 ) ) ); \
     if( dResi ) inv_trquant_tc_kernel<Nv, false><<<grid, 128, S::SMEM, ctx->stream>>>( p, dImg, dQ, n, dResi, 0, po, pp, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr ); \
     else        inv_trquant_tc_kernel<Nv, true><<<grid, 128, S::SMEM, ctx->stream>>>( p, dImg, dQ, n, nullptr, dBlocks ? 1 : 0, po, pp, dBlocks, dOrg, dPred, dReco, dRes, dSum, dLast ); }
   switch( p.w ) { case 8: VVB_ITC_CALL( 8 ) break; case 16: VVB_ITC_CALL( 16 ) break; case 32: VVB_ITC_CALL( 32 ) break; default: VVB_ITC_CALL( 64 ) break; }
@@ -1257,7 +1261,7 @@ int vvb_fwd_trquant_dev( vvb_ctx* ctx, const vvb_tu_par* par, const int16_t* dRe
   if( tc2Eligible( ctx, p ) ) return tc2Launch( ctx, p, dResi, 0, 0, nullptr, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq );
   if( !p.lfnstIdx && !p.ts && p.w == p.h && ( ( ctx->tensorTransform == 1 && ( p.w == 16 || p.w == 32 || p.w == 64 ) ) || ( ctx->tensorTransform == 2 && p.w == 64 ) ) )
   {
-    // tcgen05 path: 128 stacked rows (128/N TUs) per tile, persistent CTAs
+    // byte-plane wgmma path: 128 stacked rows (128/N TUs) per tile, persistent CTAs
     const int tpt = 128 / p.w;
     const int tiles = ( n + tpt - 1 ) / tpt;
     const int grid = std::min( tiles, ctx->numSMs * 3 );
@@ -1306,7 +1310,7 @@ int vvb_fwd_trquant_planes_dev( vvb_ctx* ctx, const vvb_tu_par* par, int orgPlan
   CU( cudaSetDevice( ctx->device ) );
   int rc;
   {
-    // CUDA-core engine: the residual is formed while the TU is loaded (one launch, no compact residual buffer); the tcgen05 engine keeps the staging kernel
+    // CUDA-core engine: the residual is formed while the TU is loaded (one launch, no compact residual buffer); the byte-plane wgmma engine keeps the staging kernel
     TuPar p;
     if( ( rc = makeTuPar( ctx, par, p ) ) ) return rc;
     if( tc2Eligible( ctx, p ) ) return tc2Launch( ctx, p, nullptr, orgPlane, predPlane, dBlocks, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq );

@@ -91,7 +91,7 @@ struct vvb_ctx
   int            pyramidEngine = 1;           // see vvb_set_pyramid_engine: 1 = all pyramid levels inside one CTA per root block, 0 = per-quad kernel + table sums
   int            useTma = 2;                  // see vvb_set_tma_staging: 0 off, 1 on, 2 (default) on where measured faster (blocks up to 8 wide)
   void*          tmaEncode = nullptr;         // cuTensorMapEncodeTiled, resolved at vvb_create
-  int            numSMs   = 148;
+  int            numSMs   = 132;
   // device-side constant data
   int8_t*        d_trTable   = nullptr;     // all transform matrices (vvc_tables.h)
   int8_t*        d_lfnst     = nullptr;     // LFNST forward kernels (vvc_lfnst_tables.h)

@@ -1,4 +1,4 @@
-// dist_kernels.cuh -- SAD / SSE / SATD (Hadamard) cost kernels for sm_100a.
+// dist_kernels.cuh -- SAD / SSE / SATD (Hadamard) cost kernels for sm_90a.
 //
 // Replaces the function-pointer surface RdCost::m_afpDistortFunc (CommonLib/RdCost.h:120, table filled at
 // CommonLib/RdCost.cpp:85-131 and overwritten by CommonLib/x86/RdCostX86.h:3376-3425).  All results are exact

@@ -1,12 +1,14 @@
-// itrquant_tc_kernels.cuh -- dequantiser + inverse 2-D transform of square TUs 8x8 .. 64x64 on the tcgen05 tensor cores, raw-byte operands as in
+// itrquant_tc_kernels.cuh -- dequantiser + inverse 2-D transform of square TUs 8x8 .. 64x64 on the wgmma tensor cores, raw-byte operands as in
 // trquant_tc2_kernels.cuh.  Simpler than the forward direction: the reference clips the dequantised coefficients and the first-pass outputs to 16 bit
 // (Quant.cpp:232-262, TrQuant_EMT.cpp fastInverse: clipMinimum / clipMaximum), so both stages read int16 values = two byte planes (low u8, high s8):
 //   stage 1 (vertical, shift 7):   A3[row (tu, column j)][2k + b] = byte b of the dequantised coefficient c[k][j]     (transposed 16-bit stores)
 //                                  B3lo[y][2k] = Tv[k][y] , B3hi[y][2k+1] = Tv[k][y]      tmp[j][y] = clip16( ( Dlo + 256 * Dhi + 64 ) >> 7 )
 //   stage 2 (horizontal, 20 - bd): A4[row (tu, y)][2j + b] = byte b of tmp[j][y]                                       (transposed 16-bit stores)
 //                                  B4lo[x][2j] = Th[j][x] , B4hi[x][2j+1] = Th[j][x]      resi[y][x] = clip16( ( Dlo + 256 * Dhi + rnd ) >> s2 )
-// Tile = 128 stage-2 rows = 128 / N TUs (at 64x64 the 64 stage-1 rows are stored twice so that the four warps share the first-pass read-back), one CTA of 128 threads, thread = one row in every phase:
-//   load + dequantise row k of the levels -> A3 ; MMA ; read (tu, j) -> clip -> A4 ; MMA ; read (tu, y) -> clip -> the residual row goes out with 16-byte stores,
+// Tile = 128 stage-2 rows = 128 / N TUs (at 64x64 the 64 stage-1 rows fill one m64 half; the threads of the other half load a copy that no MMA reads),
+// one CTA of 128 threads = one warpgroup:
+//   load + dequantise row k of the levels -> A3 ; MMA ; clip the accumulator registers -> A4 ; MMA ; clip -> staging rows ; thread = residual row (tu, y),
+//   which goes out with 16-byte stores,
 // or, for the fused TU round trip (RT), straight into reconstruction and the three distortions of tu_roundtrip_kernel (itrquant_kernels.cuh).
 // Rows / columns beyond the kept coefficients (MTS at 32 keeps 16) have zero rows in the B operands, like the loops of team_inverse that never read them.
 #pragma once
@@ -25,8 +27,8 @@ template<int N> struct ItcShape
   static constexpr int SBO = 160, LBO = 16 * SBO + 16;     // as A2 of the forward engine: the transposed stores of a warp spread over the banks
   static constexpr int A_BYTES = NCH * LBO;                // A3 and A4 have the same geometry
   static constexpr int BCH = NMMA * 16, B_BYTES = NCH * BCH;
-  static constexpr int SMEM = 2 * A_BYTES + 4 * B_BYTES;   // A3 | A4 | B3lo | B3hi | B4lo | B4hi
-  static constexpr int TMEM_COLS = 2 * NMMA < 32 ? 32 : 2 * NMMA;
+  static constexpr int LDR = N + 8;                        // int16 staging rows of the residual (16-byte aligned)
+  static constexpr int SMEM = 2 * A_BYTES + 4 * B_BYTES + 128 * LDR * 2;   // A3 | A4 | B3lo | B3hi | B4lo | B4hi | staging
   static constexpr int CH = N < 16 ? 8 : 16;
 };
 
@@ -59,29 +61,15 @@ __global__ void __launch_bounds__( 128, 4 ) inv_trquant_tc_kernel( const __grid_
   unsigned char* sA3 = smemItc;
   unsigned char* sA4 = smemItc + S::A_BYTES;
   unsigned char* sB  = smemItc + 2 * S::A_BYTES;
-  __shared__ __align__( 8 ) unsigned long long sMbar;
-  __shared__ uint32_t sTmemBase;
+  int16_t* sR = reinterpret_cast<int16_t*>( sB + 4 * S::B_BYTES );
 
   const int tid = threadIdx.x, warp = tid >> 5;
-  const uint32_t mbar = smem_u32( &sMbar );
-  if( warp == 0 )
-  {
-    asm volatile( "tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"( smem_u32( &sTmemBase ) ), "r"( (uint32_t) S::TMEM_COLS ) : "memory" );
-    asm volatile( "tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory" );
-  }
-  if( tid == 0 ) { mbar_init( mbar, 1 ); asm volatile( "fence.mbarrier_init.release.cluster;" ::: "memory" ); }
   for( int i = tid; i < 4 * S::B_BYTES / 16; i += 128 ) reinterpret_cast<uint4*>( sB )[i] = __ldg( bImage + i );
   for( int i = tid; i < 2 * S::A_BYTES / 16; i += 128 ) reinterpret_cast<uint4*>( sA3 )[i] = make_uint4( 0, 0, 0, 0 );     // K padding (8x8) stays zero
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = sTmemBase;
-  uint32_t phase = 0;
-  const uint32_t idescU = umma_idesc_i8_a( 128, NMMA, 0 ), idescS = umma_idesc_i8_a( 128, NMMA, 1 );
-  const uint64_t dA3 = umma_desc_kmajor( smem_u32( sA3 ), S::LBO, S::SBO ), dA4 = umma_desc_kmajor( smem_u32( sA4 ), S::LBO, S::SBO );
-  const uint64_t dB = umma_desc_kmajor( smem_u32( sB ), S::BCH, 128 );
+  const uint64_t dA3 = gmma_desc_kmajor( smem_u32( sA3 ), S::LBO, S::SBO ), dA4 = gmma_desc_kmajor( smem_u32( sA4 ), S::LBO, S::SBO );
+  const uint64_t dB = gmma_desc_kmajor( smem_u32( sB ), S::BCH, 128 );
   const int numTiles = ( n + TPT - 1 ) / TPT;
-  const uint32_t laneBase = (uint32_t)( warp * 32 ) << 16;
   const int tl = tid / N, rr = tid % N;                       // stage 2: TU of the tile and row y of this thread
   const int r1 = tid % KEEP, t1 = ( tid / KEEP ) % TPT, cp = tid / ( KEEP * TPT );   // levels / stage 1: row k resp. column j, TU, copy (64x64 only)
   const int sc = par.dqScale, sh = par.dqShift, inMax = par.dqInMax, inMin = -inMax - 1;
@@ -89,7 +77,6 @@ __global__ void __launch_bounds__( 128, 4 ) inv_trquant_tc_kernel( const __grid_
   const int s2 = par.s2Inv, r2 = 1 << ( s2 - 1 );
   // transposed 16-bit store of element e (0..N-1) of this thread's row into row (tl, e) of an A operand, K position rr
   unsigned char* const stBase3 = sA3 + ( r1 >> 3 ) * S::LBO + ( ( cp * TPT + t1 ) * KEEP / 8 ) * S::SBO + ( r1 & 7 ) * 2;
-  unsigned char* const stBase4 = sA4 + ( r1 >> 3 ) * S::LBO + ( t1 * N / 8 ) * S::SBO + ( r1 & 7 ) * 2;
 
   for( int tile = blockIdx.x; tile < numTiles; tile += gridDim.x )
   {
@@ -121,56 +108,66 @@ __global__ void __launch_bounds__( 128, 4 ) inv_trquant_tc_kernel( const __grid_
     }
     fence_async_smem();
     __syncthreads();
-    if( tid == 0 )
+    // ---- stage 1: Dlo / Dhi [rows (t1, column j) x y] (A3 read as u8 / s8); tmp[j][y] = clip16( ( Dlo + 256 * Dhi + 64 ) >> 7 ) -> A4 row (t1, y), K position j
     {
-      tc_fence_after();
+      constexpr int MH = DUP == 2 ? 1 : 2;                     // 64x64: the copy in rows 64..127 is not multiplied
+      int lo[MH][NMMA / 2], hi[MH][NMMA / 2];
 #pragma unroll
-      for( int p = 0; p < 2; p++ )
+      for( int h = 0; h < MH; h++ ) { wg_hold( lo[h] ); wg_hold( hi[h] ); }
+      wg_fence();
+#pragma unroll
+      for( int h = 0; h < MH; h++ )
 #pragma unroll
         for( int ks = 0; ks < S::K / 32; ks++ )
-          umma_i8( tmem + p * NMMA, dA3 + (uint64_t)( ( ks * 2 * S::LBO ) >> 4 ), dB + (uint64_t)( ( p * S::B_BYTES + ks * 2 * S::BCH ) >> 4 ), p ? idescS : idescU, ks > 0 ? 1u : 0u );
-      umma_commit( mbar );
-      mbar_wait_hint( mbar, phase );
-    }
-    phase ^= 1;
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    // ---- first-pass outputs of column j = r1 of TU t1 (lane = stage-1 row): tmp[j][y] -> A4 row (t1, y), K position j; copy cp takes the y of its half
+        {
+          const uint64_t da = dA3 + (uint64_t)( ( h * 8 * S::SBO + ks * 2 * S::LBO ) >> 4 );
+          wgmma_i8<NMMA, false>( lo[h], da, dB + (uint64_t)( ( ks * 2 * S::BCH ) >> 4 ), ks > 0 );
+          wgmma_i8<NMMA, true>( hi[h], da, dB + (uint64_t)( ( S::B_BYTES + ks * 2 * S::BCH ) >> 4 ), ks > 0 );
+        }
+      wg_commit();
+      wg_wait0();
 #pragma unroll
-    for( int c0 = 0; c0 < N / DUP; c0 += CH )
-    {
-      const int yb = cp * ( N / DUP ) + c0;
-      int lo[CH], hi[CH];
-      tmem_ldc<CH>( tmem + laneBase + yb, lo );
-      tmem_ldc<CH>( tmem + laneBase + NMMA + yb, hi );
-      tmem_ld_wait();
+      for( int h = 0; h < MH; h++ ) { wg_hold( lo[h] ); wg_hold( hi[h] ); }
 #pragma unroll
-      for( int k = 0; k < CH; k++ )
-      {
-        const int y = yb + k;
-        const int t = clip16( ( ( hi[k] << 8 ) + lo[k] + 64 ) >> 7 );
-        *reinterpret_cast<int16_t*>( stBase4 + ( y >> 3 ) * S::SBO + ( y & 7 ) * 16 ) = (int16_t) t;
-      }
+      for( int h = 0; h < MH; h++ )
+#pragma unroll
+        for( int i = 0; i < NMMA / 2; i++ )
+        {
+          const int r = h * 64 + wg_row( i ), y = wg_col( i ), j = r % KEEP, t = ( r / KEEP ) % TPT;
+          if( y < N )
+            *reinterpret_cast<int16_t*>( sA4 + ( j >> 3 ) * S::LBO + ( t * N / 8 + ( y >> 3 ) ) * S::SBO + ( j & 7 ) * 2 + ( y & 7 ) * 16 ) =
+              (int16_t) clip16( ( ( hi[h][i] << 8 ) + lo[h][i] + 64 ) >> 7 );
+        }
     }
-    tc_fence_before();
     fence_async_smem();
     __syncthreads();
-    if( tid == 0 )
+    // ---- stage 2: rows (tu, y) x columns x (A4 read as u8 / s8), one 64-row half at a time, each with accumulators of its own;
+    //      resi = clip16( ( Dlo + 256 * Dhi + rnd ) >> s2 ) -> staging
     {
-      tc_fence_after();
+      int lo[2][NMMA / 2], hi[2][NMMA / 2];
 #pragma unroll
-      for( int p = 0; p < 2; p++ )
+      for( int h = 0; h < 2; h++ )
+      {
+        wg_fence();
 #pragma unroll
         for( int ks = 0; ks < S::K / 32; ks++ )
-          umma_i8( tmem + p * NMMA, dA4 + (uint64_t)( ( ks * 2 * S::LBO ) >> 4 ), dB + (uint64_t)( ( ( 2 + p ) * S::B_BYTES + ks * 2 * S::BCH ) >> 4 ), p ? idescS : idescU, ks > 0 ? 1u : 0u );
-      umma_commit( mbar );
-      mbar_wait_hint( mbar, phase );
+        {
+          const uint64_t da = dA4 + (uint64_t)( ( h * 8 * S::SBO + ks * 2 * S::LBO ) >> 4 );
+          wgmma_i8<NMMA, false>( lo[h], da, dB + (uint64_t)( ( 2 * S::B_BYTES + ks * 2 * S::BCH ) >> 4 ), ks > 0 );
+          wgmma_i8<NMMA, true>( hi[h], da, dB + (uint64_t)( ( 3 * S::B_BYTES + ks * 2 * S::BCH ) >> 4 ), ks > 0 );
+        }
+        wg_commit();
+        wg_wait0();
+        wg_hold( lo[h] ); wg_hold( hi[h] );
+#pragma unroll
+        for( int i = 0; i < NMMA / 2; i++ )
+        {
+          const int r = h * 64 + wg_row( i ), x = wg_col( i );
+          if( x < N ) sR[r * S::LDR + x] = (int16_t) clip16( ( ( hi[h][i] << 8 ) + lo[h][i] + r2 ) >> s2 );
+        }
+      }
     }
-    phase ^= 1;
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
     // ---- residual row y = rr
     {
       int16_t* dst = RT ? nullptr : resiOut + ( (size_t)( live ? tu : 0 ) * N + rr ) * N;
@@ -195,13 +192,15 @@ __global__ void __launch_bounds__( 128, 4 ) inv_trquant_tc_kernel( const __grid_
 #pragma unroll
       for( int c0 = 0; c0 < N; c0 += CH )
       {
-        int lo[CH], hi[CH];
-        tmem_ldc<CH>( tmem + laneBase + c0, lo );
-        tmem_ldc<CH>( tmem + laneBase + NMMA + c0, hi );
-        tmem_ld_wait();
         int r[CH];
 #pragma unroll
-        for( int k = 0; k < CH; k++ ) r[k] = active ? clip16( ( ( hi[k] << 8 ) + lo[k] + r2 ) >> s2 ) : 0;
+        for( int k = 0; k < CH; k += 8 )
+        {
+          const uint4 v = *reinterpret_cast<const uint4*>( sR + tid * S::LDR + c0 + k );
+          const uint32_t w[4] = { v.x, v.y, v.z, v.w };
+#pragma unroll
+          for( int e = 0; e < 8; e++ ) r[k + e] = active ? ( e & 1 ? hi16( w[e >> 1] ) : lo16( w[e >> 1] ) ) : 0;
+        }
         if( !RT )
         {
           if( live )
@@ -262,12 +261,8 @@ __global__ void __launch_bounds__( 128, 4 ) inv_trquant_tc_kernel( const __grid_
         }
       }
     }
-    tc_fence_before();
     __syncthreads();
   }
-  tc_fence_before();
-  __syncthreads();
-  if( warp == 0 ) asm volatile( "tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"( tmem ), "r"( (uint32_t) S::TMEM_COLS ) : "memory" );
 }
 
 } // namespace vvb

@@ -1,4 +1,4 @@
-// mctf_affine_kernels.cuh -- MCTF block-matching errors and affine-ME gradient helpers for sm_100a.
+// mctf_affine_kernels.cuh -- MCTF block-matching errors and affine-ME gradient helpers for sm_90a.
 //
 // MCTF: MCTF::motionErrorLuma (CommonLib/MCTF.cpp:1099-1164) -> motionErrorLumaInt (:122-145),
 //       motionErrorLumaFrac6 (:147-203), motionErrorLumaFrac4 (:205-257); filter tables :72-110.

@@ -1,4 +1,4 @@
-// pyramid_kernels.cuh -- SAD pyramid of the dense integer search with every level formed inside one CTA (sm_100a).
+// pyramid_kernels.cuh -- SAD pyramid of the dense integer search with every level formed inside one CTA (sm_90a).
 //
 // Replaces, for 8x8 base blocks without row sub-sampling, the pair sad_search_kernel<.., PARENT> + sad_table_sum_kernel: one CTA owns one ROOT block of
 // 16x16, 32x32 or 64x64 pels (LV = 2, 3, 4 levels) together with all of its quad-tree descendants, stages the reference window of the whole root once and
@@ -9,7 +9,7 @@
 //
 // Arithmetic per (8x8 block, candidate):  SAD = sum a + sum b - 2 sum min(a,b)
 //   sum a : per block, once;  sum b : 8x8 box sums of the window (uint16 table V);  sum min : VIMNMX.S16x2 (alu pipe) + IDP.2A (fma pipe) per pel pair.
-// Both pipes issue every other cycle per scheduler (B300_MICROARCH.md "fma vs alu split"), so one min + one dot product per pel pair is the floor of this
+// Both pipes accept a warp instruction every other cycle per scheduler, so one min + one dot product per pel pair is the floor of this
 // formulation; everything else is kept off the alu pipe where possible:
 //   * odd-offset candidates read a second, one-pel-shifted copy of the window (no funnel shifts),
 //   * a thread evaluates TWO vertically adjacent candidate rows for a strip of 8 vectors: the nine window rows they need are loaded once (LDS.128) and

@@ -1,4 +1,4 @@
-// search_kernels.cuh -- integer motion-search SAD sweeps for sm_100a.
+// search_kernels.cuh -- integer motion-search SAD sweeps for sm_90a.
 //
 //  * sad_search_kernel : dense full search, InterSearch::xPatternSearch (EncoderLib/InterSearch.cpp:2209-2251).
 //    One CTA per block; the (w + range) x (h + range) reference window and the original block are staged in shared

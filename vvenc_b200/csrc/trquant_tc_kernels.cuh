@@ -1,4 +1,4 @@
-// trquant_tc_kernels.cuh -- forward 2-D integer transform on the 5th-generation tensor cores (tcgen05, kind::i8, TMEM
+// trquant_tc_kernels.cuh -- forward 2-D integer transform on the Hopper tensor cores (wgmma, s8 x s8 -> s32, register
 // accumulators) + the same fused quantiser as trquant_kernels.cuh.  Square TUs 16x16, 32x32, 64x64.
 //
 // Exact-integer strategy (SURVEY.md 7-3): the transform is pure int32 (TrQuant_EMT.cpp:1973-2000), the matrices fit s8
@@ -10,8 +10,8 @@
 //
 // Tile = 128 stacked rows = 128/N TUs.  A operands are written to shared memory by the threads themselves in the canonical
 // K-major no-swizzle layout ([16-byte K chunk][row][16 B]: SBO = 128 B, LBO = rows*16 B), B = the transform matrix rows in
-// the same layout, D lives in TMEM (lane = stacked row, column = output index).  Stage-1 results are scattered transposed
-// (bytes) into the stage-2 A operand, so the second transform is again "rows x matrix".
+// the same layout, D lives in the registers of the warpgroup (two m64 halves of the 128 rows).  Stage-1 results are scattered
+// transposed (bytes) into the stage-2 A operand, so the second transform is again "rows x matrix".
 #pragma once
 #include "common.cuh"
 #include "trquant_kernels.cuh"
@@ -20,74 +20,77 @@ namespace vvb {
 
 __device__ __forceinline__ uint32_t smem_u32( const void* p ) { return (uint32_t) __cvta_generic_to_shared( p ); }
 
-// UMMA shared-memory descriptor, K-major, SWIZZLE_NONE (cute/arch/mma_sm100_desc.hpp SmemDescriptor; cute/atom/mma_traits_sm100.hpp:273-303)
-__device__ __forceinline__ uint64_t umma_desc_kmajor( uint32_t smemAddr, uint32_t lboBytes, uint32_t sboBytes )
+// wgmma shared-memory descriptor, K-major, no swizzle (PTX ISA, "Matrix Descriptor Format"): start address, leading byte offset = stride between the
+// 16-byte K chunks of a k32 step, stride byte offset = stride between 8-row groups; base offset 0, layout type 0
+__device__ __forceinline__ uint64_t gmma_desc_kmajor( uint32_t smemAddr, uint32_t lboBytes, uint32_t sboBytes )
 {
   uint64_t d = 0;
   d |= (uint64_t)( ( smemAddr >> 4 ) & 0x3fffu );           // start address, bits [0,14)
   d |= (uint64_t)( ( lboBytes >> 4 ) & 0x3fffu ) << 16;     // leading byte offset, bits [16,30)
   d |= (uint64_t)( ( sboBytes >> 4 ) & 0x3fffu ) << 32;     // stride byte offset, bits [32,46)
-  d |= (uint64_t) 1 << 46;                                   // version = 1 (sm_100)
-  return d;                                                  // base_offset 0, lbo_mode 0, layout_type 0 (no swizzle)
-}
-
-// UMMA instruction descriptor for kind::i8, s8 x s8 -> s32, both operands K-major (mma_sm100_desc.hpp InstrDescriptor)
-__device__ __forceinline__ uint32_t umma_idesc_i8( int M, int N )
-{
-  uint32_t d = 0;
-  d |= 2u << 4;                      // c_format = S32
-  d |= 1u << 7;                      // a_format = INT8 (signed)
-  d |= 1u << 10;                     // b_format = INT8 (signed)
-  d |= (uint32_t)( N >> 3 ) << 17;   // n_dim
-  d |= (uint32_t)( M >> 4 ) << 24;   // m_dim
   return d;
 }
 
-__device__ __forceinline__ void umma_i8( uint32_t tmemD, uint64_t descA, uint64_t descB, uint32_t idesc, uint32_t accumulate )
+// D[64 x NN] (+)= A[64 x 32 B] * B[NN x 32 B]^T, A read as u8 (AS = false) or s8 (AS = true), B as s8, s32 accumulators; issued by the whole warpgroup
+// (the 128 threads of the CTA).  accumulate = 0 starts the chain.  Register i of a thread holds row wg_row( i ), column wg_col( i ) of D.
+template<int NN, bool AS> __device__ __forceinline__ void wgmma_i8( int (&d)[NN / 2], uint64_t descA, uint64_t descB, int accumulate );
+template<> __device__ __forceinline__ void wgmma_i8<16, false>( int (&d)[8], uint64_t descA, uint64_t descB, int accumulate )
 {
-  asm volatile(
-    "{\n\t"
-    ".reg .pred p;\n\t"
-    "setp.ne.b32 p, %4, 0;\n\t"
-    "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, {%5, %6, %7, %8}, p;\n\t"
-    "}\n"
-    :: "r"( tmemD ), "l"( descA ), "l"( descB ), "r"( idesc ), "r"( accumulate ), "r"( 0u ), "r"( 0u ), "r"( 0u ), "r"( 0u ) : "memory" );
+  asm volatile( "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+                "wgmma.mma_async.sync.aligned.m64n16k32.s32.u8.s8 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p;\n\t}\n"
+                : "+r"( d[0] ), "+r"( d[1] ), "+r"( d[2] ), "+r"( d[3] ), "+r"( d[4] ), "+r"( d[5] ), "+r"( d[6] ), "+r"( d[7] )
+                : "l"( descA ), "l"( descB ), "r"( accumulate ) : "memory" );
+}
+template<> __device__ __forceinline__ void wgmma_i8<16, true>( int (&d)[8], uint64_t descA, uint64_t descB, int accumulate )
+{
+  asm volatile( "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+                "wgmma.mma_async.sync.aligned.m64n16k32.s32.s8.s8 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p;\n\t}\n"
+                : "+r"( d[0] ), "+r"( d[1] ), "+r"( d[2] ), "+r"( d[3] ), "+r"( d[4] ), "+r"( d[5] ), "+r"( d[6] ), "+r"( d[7] )
+                : "l"( descA ), "l"( descB ), "r"( accumulate ) : "memory" );
+}
+template<> __device__ __forceinline__ void wgmma_i8<32, false>( int (&d)[16], uint64_t descA, uint64_t descB, int accumulate )
+{
+  asm volatile( "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+                "wgmma.mma_async.sync.aligned.m64n32k32.s32.u8.s8 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p;\n\t}\n"
+                : "+r"( d[0] ), "+r"( d[1] ), "+r"( d[2] ), "+r"( d[3] ), "+r"( d[4] ), "+r"( d[5] ), "+r"( d[6] ), "+r"( d[7] ), "+r"( d[8] ), "+r"( d[9] ), "+r"( d[10] ), "+r"( d[11] ), "+r"( d[12] ), "+r"( d[13] ), "+r"( d[14] ), "+r"( d[15] )
+                : "l"( descA ), "l"( descB ), "r"( accumulate ) : "memory" );
+}
+template<> __device__ __forceinline__ void wgmma_i8<32, true>( int (&d)[16], uint64_t descA, uint64_t descB, int accumulate )
+{
+  asm volatile( "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+                "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p;\n\t}\n"
+                : "+r"( d[0] ), "+r"( d[1] ), "+r"( d[2] ), "+r"( d[3] ), "+r"( d[4] ), "+r"( d[5] ), "+r"( d[6] ), "+r"( d[7] ), "+r"( d[8] ), "+r"( d[9] ), "+r"( d[10] ), "+r"( d[11] ), "+r"( d[12] ), "+r"( d[13] ), "+r"( d[14] ), "+r"( d[15] )
+                : "l"( descA ), "l"( descB ), "r"( accumulate ) : "memory" );
+}
+template<> __device__ __forceinline__ void wgmma_i8<64, false>( int (&d)[32], uint64_t descA, uint64_t descB, int accumulate )
+{
+  asm volatile( "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                "wgmma.mma_async.sync.aligned.m64n64k32.s32.u8.s8 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p;\n\t}\n"
+                : "+r"( d[0] ), "+r"( d[1] ), "+r"( d[2] ), "+r"( d[3] ), "+r"( d[4] ), "+r"( d[5] ), "+r"( d[6] ), "+r"( d[7] ), "+r"( d[8] ), "+r"( d[9] ), "+r"( d[10] ), "+r"( d[11] ), "+r"( d[12] ), "+r"( d[13] ), "+r"( d[14] ), "+r"( d[15] ), "+r"( d[16] ), "+r"( d[17] ), "+r"( d[18] ), "+r"( d[19] ), "+r"( d[20] ), "+r"( d[21] ), "+r"( d[22] ), "+r"( d[23] ), "+r"( d[24] ), "+r"( d[25] ), "+r"( d[26] ), "+r"( d[27] ), "+r"( d[28] ), "+r"( d[29] ), "+r"( d[30] ), "+r"( d[31] )
+                : "l"( descA ), "l"( descB ), "r"( accumulate ) : "memory" );
+}
+template<> __device__ __forceinline__ void wgmma_i8<64, true>( int (&d)[32], uint64_t descA, uint64_t descB, int accumulate )
+{
+  asm volatile( "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p;\n\t}\n"
+                : "+r"( d[0] ), "+r"( d[1] ), "+r"( d[2] ), "+r"( d[3] ), "+r"( d[4] ), "+r"( d[5] ), "+r"( d[6] ), "+r"( d[7] ), "+r"( d[8] ), "+r"( d[9] ), "+r"( d[10] ), "+r"( d[11] ), "+r"( d[12] ), "+r"( d[13] ), "+r"( d[14] ), "+r"( d[15] ), "+r"( d[16] ), "+r"( d[17] ), "+r"( d[18] ), "+r"( d[19] ), "+r"( d[20] ), "+r"( d[21] ), "+r"( d[22] ), "+r"( d[23] ), "+r"( d[24] ), "+r"( d[25] ), "+r"( d[26] ), "+r"( d[27] ), "+r"( d[28] ), "+r"( d[29] ), "+r"( d[30] ), "+r"( d[31] )
+                : "l"( descA ), "l"( descB ), "r"( accumulate ) : "memory" );
 }
 
-__device__ __forceinline__ void umma_commit( uint32_t mbarAddr )
-{
-  asm volatile( "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"( mbarAddr ) : "memory" );
-}
 
-__device__ __forceinline__ void mbar_init( uint32_t addr, uint32_t count ) { asm volatile( "mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"( addr ), "r"( count ) : "memory" ); }
-
-__device__ __forceinline__ void mbar_wait( uint32_t addr, uint32_t parity )
+__device__ __forceinline__ int wg_row( int i ) { return ( ( threadIdx.x >> 5 ) << 4 ) + ( ( threadIdx.x & 31 ) >> 2 ) + ( i & 2 ) * 4; }
+__device__ __forceinline__ int wg_col( int i ) { return ( i >> 2 ) * 8 + ( threadIdx.x & 3 ) * 2 + ( i & 1 ); }
+__device__ __forceinline__ void wg_fence()  { asm volatile( "wgmma.fence.sync.aligned;" ::: "memory" ); }
+__device__ __forceinline__ void wg_commit() { asm volatile( "wgmma.commit_group.sync.aligned;" ::: "memory" ); }
+__device__ __forceinline__ void wg_wait0()  { asm volatile( "wgmma.wait_group.sync.aligned 0;" ::: "memory" ); }
+// the compiler does not know that wgmma writes its accumulator registers asynchronously: pinning every register here (before the first MMA of a group
+// and after wgmma.wait_group) keeps it from reading, moving or reusing them while MMAs are in flight
+template<int R> __device__ __forceinline__ void wg_hold( int (&d)[R] )
 {
-  uint32_t done = 0;
-  while( !done )
-  {
-    asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t"
-      "}\n" : "=r"( done ) : "r"( addr ), "r"( parity ) : "memory" );
-  }
+#pragma unroll
+  for( int i = 0; i < R; i++ ) asm volatile( "" : "+r"( d[i] ) :: "memory" );
 }
-
-__device__ __forceinline__ void tmem_ld16( uint32_t taddr, int (&v)[16] )
-{
-  asm volatile( "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                : "=r"( v[0] ), "=r"( v[1] ), "=r"( v[2] ), "=r"( v[3] ), "=r"( v[4] ), "=r"( v[5] ), "=r"( v[6] ), "=r"( v[7] ),
-                  "=r"( v[8] ), "=r"( v[9] ), "=r"( v[10] ), "=r"( v[11] ), "=r"( v[12] ), "=r"( v[13] ), "=r"( v[14] ), "=r"( v[15] )
-                : "r"( taddr ) : "memory" );
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile( "tcgen05.wait::ld.sync.aligned;" ::: "memory" ); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile( "tcgen05.fence::before_thread_sync;" ::: "memory" ); }
-__device__ __forceinline__ void tc_fence_after()  { asm volatile( "tcgen05.fence::after_thread_sync;" ::: "memory" ); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile( "fence.proxy.async.shared::cta;" ::: "memory" ); }
-
-#define TC_TMEM_COLS 128
 
 // N = TU size (16, 32, 64).  KB = bytes of K per operand row = max(32, N); KEEP = N > 32 ? 32 : N (zero-out, DCT-II only at 64).
 template<int N>
@@ -111,20 +114,11 @@ __global__ void __launch_bounds__( 128 ) fwd_trquant_tc_kernel( const __grid_con
   int32_t*       sCoef = reinterpret_cast<int32_t*>( sBv + B_BYTES );          // [TPT][REGION]
   uint32_t*      sQ    = reinterpret_cast<uint32_t*>( sCoef + TPT * REGION );  // [TPT][N*N/2] int16 pairs (levels)
   int*           sRed  = reinterpret_cast<int*>( sQ + TPT * N * N / 2 );       // [TPT][8]
-  __shared__ __align__( 8 ) unsigned long long sMbar;
-  __shared__ uint32_t sTmemBase;
 
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int keepW = par.keepW, keepH = par.keepH;            // == KEEP for DCT-II; 16 for DST-VII/DCT-VIII at 32
-  const uint32_t mbar = smem_u32( &sMbar );
 
-  // ---- one-time set-up: TMEM allocation (warp 0), barrier init, matrices in canonical layout
-  if( warp == 0 )
-  {
-    asm volatile( "tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"( smem_u32( &sTmemBase ) ), "r"( (uint32_t) TC_TMEM_COLS ) : "memory" );
-    asm volatile( "tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory" );
-  }
-  if( tid == 0 ) { mbar_init( mbar, 1 ); asm volatile( "fence.mbarrier_init.release.cluster;" ::: "memory" ); }
+  // ---- one-time set-up: matrices in canonical layout
   // B[chunk c][row j (0..31)][16 B] = T[j][16c .. 16c+15], zero beyond N (K padding) and beyond the kept rows
   for( int i = tid; i < NCH * 32 * 16; i += 128 )
   {
@@ -132,13 +126,9 @@ __global__ void __launch_bounds__( 128 ) fwd_trquant_tc_kernel( const __grid_con
     sBh[i] = ( r < keepW && k < N ) ? (unsigned char) trTable[par.offH + r * N + k] : 0;
     sBv[i] = ( r < keepH && k < N ) ? (unsigned char) trTable[par.offV + r * N + k] : 0;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = sTmemBase;
-  uint32_t phase = 0;
 
-  const uint32_t idesc = umma_idesc_i8( 128, 32 );           // N operand padded to 32 columns for every TU size (rows >= keep are zero)
+  // the N operand is padded to 32 columns for every TU size (rows >= keep are zero)
   const uint32_t aAddr = smem_u32( sA ), bhAddr = smem_u32( sBh ), bvAddr = smem_u32( sBv );
   const int numTiles = ( n + TPT - 1 ) / TPT;
   const int r1 = par.s1 > 0 ? 1 << ( par.s1 - 1 ) : 0, r2 = 1 << ( par.s2 - 1 );
@@ -182,103 +172,78 @@ __global__ void __launch_bounds__( 128 ) fwd_trquant_tc_kernel( const __grid_con
     }
     fence_async_smem();
     __syncthreads();
-    // ---- stage-1 MMAs: D_p[128 x 32] (columns 32p..) = A_p[128 x KB] * Bh^T, p = 0,1
-    if( tid == 0 )
-    {
-      tc_fence_after();
+    // ---- stage-1 MMAs: D_p[128 x 32] (d[half][p]) = A_p[128 x KB] * Bh^T, p = 0,1
+    int d[2][2][16];
+    wg_hold( d[0][0] ); wg_hold( d[0][1] ); wg_hold( d[1][0] ); wg_hold( d[1][1] );
+    wg_fence();
+#pragma unroll
+    for( int h = 0; h < 2; h++ )
 #pragma unroll
       for( int p = 0; p < 2; p++ )
 #pragma unroll
         for( int ks = 0; ks < KB / 32; ks++ )
         {
-          const uint64_t da = umma_desc_kmajor( aAddr + p * A_BYTES + ks * 2 * 128 * 16, 128 * 16, 128 );
-          const uint64_t db = umma_desc_kmajor( bhAddr + ks * 2 * 32 * 16, 32 * 16, 128 );
-          umma_i8( tmem + 32 * p, da, db, idesc, ks > 0 ? 1u : 0u );
+          const uint64_t da = gmma_desc_kmajor( aAddr + p * A_BYTES + h * 64 * 16 + ks * 2 * 128 * 16, 128 * 16, 128 );
+          const uint64_t db = gmma_desc_kmajor( bhAddr + ks * 2 * 32 * 16, 32 * 16, 128 );
+          wgmma_i8<32, true>( d[h][p], da, db, ks > 0 );
         }
-      umma_commit( mbar );
-    }
-    mbar_wait( mbar, phase ); phase ^= 1;
-    tc_fence_after();
+    wg_commit();
+    wg_wait0();
+    wg_hold( d[0][0] ); wg_hold( d[0][1] ); wg_hold( d[1][0] ); wg_hold( d[1][1] );
+    __syncthreads();                                     // every MMA has read its A rows
     // ---- stage-1 epilogue: tmp[i][j] = ((d1 << 7) + d0 + r1) >> s1 ; scatter three byte planes, transposed, as stage-2 A
     {
-      const uint32_t lane = (uint32_t)( warp * 32 ) << 16;
       // zero the three planes first (rows of TUs that keep fewer columns, K padding) -- each thread clears its own rows
 #pragma unroll
       for( int p = 0; p < 3; p++ )
 #pragma unroll
         for( int c = 0; c < NCH; c++ ) *reinterpret_cast<uint4*>( sA + p * A_BYTES + ( c * 128 + tid ) * 16 ) = make_uint4( 0, 0, 0, 0 );
-      int d0[16], d1[16];
-      int tmpv[32];
+      __syncthreads();
 #pragma unroll
-      for( int half = 0; half < 2; half++ )
-      {
-        tmem_ld16( tmem + lane + 0  + 16 * half, d0 );
-        tmem_ld16( tmem + lane + 32 + 16 * half, d1 );
-        tmem_ld_wait();
+      for( int h = 0; h < 2; h++ )
 #pragma unroll
-        for( int j = 0; j < 16; j++ ) tmpv[16 * half + j] = ( ( d1[j] << 7 ) + d0[j] + r1 ) >> par.s1;
-      }
-      tc_fence_before();
-      __syncthreads();                                   // every row's old A bytes are consumed and cleared before the scatter
-      if( live )
-      {
-        // stage-2 stacked row = tuInTile * keepW + j ; K index = rowInTu
-        const int c = rowInTu >> 4, b = rowInTu & 15;
-#pragma unroll
-        for( int j = 0; j < 32; j++ )
+        for( int i = 0; i < 16; i++ )
         {
-          if( j < keepW )
+          // stage-1 row = (TU row / N, row in TU) ; stage-2 stacked row = tuInTile * keepW + j ; K index = row in TU
+          const int row = h * 64 + wg_row( i ), j = wg_col( i ), rt = row % N;
+          if( j < keepW && tile * TPT + row / N < n )
           {
-            const int t = tmpv[j];
-            const int row2 = tuInTile * keepW + j;
-            unsigned char* dst = sA + ( c * 128 + row2 ) * 16 + b;
+            const int t = ( ( d[h][1][i] << 7 ) + d[h][0][i] + r1 ) >> par.s1;
+            unsigned char* dst = sA + ( ( rt >> 4 ) * 128 + ( row / N ) * keepW + j ) * 16 + ( rt & 15 );
             dst[0 * A_BYTES] = (unsigned char)( t & 127 );
             dst[1 * A_BYTES] = (unsigned char)( ( t >> 7 ) & 127 );
             dst[2 * A_BYTES] = (unsigned char)( ( t >> 14 ) & 255 );
           }
         }
-      }
     }
     fence_async_smem();
     __syncthreads();
-    // ---- stage-2 MMAs: D_p[128 x 32] = A2_p * Bv^T, p = 0,1,2
-    if( tid == 0 )
-    {
-      tc_fence_after();
-#pragma unroll
-      for( int p = 0; p < 3; p++ )
-#pragma unroll
-        for( int ks = 0; ks < KB / 32; ks++ )
-        {
-          const uint64_t da = umma_desc_kmajor( aAddr + p * A_BYTES + ks * 2 * 128 * 16, 128 * 16, 128 );
-          const uint64_t db = umma_desc_kmajor( bvAddr + ks * 2 * 32 * 16, 32 * 16, 128 );
-          umma_i8( tmem + 32 * p, da, db, idesc, ks > 0 ? 1u : 0u );
-        }
-      umma_commit( mbar );
-    }
-    mbar_wait( mbar, phase ); phase ^= 1;
-    tc_fence_after();
+    // ---- stage-2 MMAs: D_p[128 x 32] = A2_p * Bv^T, p = 0,1,2, one 64-row half at a time
     // ---- stage-2 epilogue: stacked row = (TU t2, column i') ; coef[j'][i'] = ((d2<<14) + (d1<<7) + d0 + r2) >> s2
     {
-      const uint32_t lane = (uint32_t)( warp * 32 ) << 16;
-      const int t2 = tid / keepW, i2 = tid - t2 * keepW;
-      const bool rowLive = t2 < TPT && ( tile * TPT + t2 ) < n;
-      int d0[16], d1[16], d2[16];
 #pragma unroll
-      for( int half = 0; half < 2; half++ )
+      for( int h = 0; h < 2; h++ )
       {
-        tmem_ld16( tmem + lane + 0  + 16 * half, d0 );
-        tmem_ld16( tmem + lane + 32 + 16 * half, d1 );
-        tmem_ld16( tmem + lane + 64 + 16 * half, d2 );
-        tmem_ld_wait();
-        if( rowLive )
-        {
+        int e[3][16];
+        wg_hold( e[0] ); wg_hold( e[1] ); wg_hold( e[2] );
+        wg_fence();
 #pragma unroll
-          for( int j = 0; j < 16; j++ )
+        for( int p = 0; p < 3; p++ )
+#pragma unroll
+          for( int ks = 0; ks < KB / 32; ks++ )
           {
-            const int jj = 16 * half + j;
-            if( jj < keepH ) sCoef[t2 * REGION + jj * KEEP + i2] = ( ( d2[j] << 14 ) + ( d1[j] << 7 ) + d0[j] + r2 ) >> par.s2;
+            const uint64_t da = gmma_desc_kmajor( aAddr + p * A_BYTES + h * 64 * 16 + ks * 2 * 128 * 16, 128 * 16, 128 );
+            const uint64_t db = gmma_desc_kmajor( bvAddr + ks * 2 * 32 * 16, 32 * 16, 128 );
+            wgmma_i8<32, true>( e[p], da, db, ks > 0 );
           }
+        wg_commit();
+        wg_wait0();
+        wg_hold( e[0] ); wg_hold( e[1] ); wg_hold( e[2] );
+#pragma unroll
+        for( int i = 0; i < 16; i++ )
+        {
+          const int row = h * 64 + wg_row( i ), jj = wg_col( i ), t2 = row / keepW, i2 = row - t2 * keepW;
+          if( t2 < TPT && tile * TPT + t2 < n && jj < keepH ) sCoef[t2 * REGION + jj * KEEP + i2] = ( ( e[2][i] << 14 ) + ( e[1][i] << 7 ) + e[0][i] + r2 ) >> par.s2;
         }
       }
       // MTS at 32 keeps 16x16 of the 32x32 scan region: clear the rest
@@ -289,7 +254,6 @@ __global__ void __launch_bounds__( 128 ) fwd_trquant_tc_kernel( const __grid_con
           if( cc >= keepW || rr >= keepH ) sCoef[i] = 0;
         }
     }
-    tc_fence_before();
     __syncthreads();
 
     // ---- quantiser: the same device function as the CUDA-core kernel, team of N threads per TU
@@ -323,11 +287,6 @@ __global__ void __launch_bounds__( 128 ) fwd_trquant_tc_kernel( const __grid_con
     }
     __syncthreads();
   }
-
-  // ---- teardown
-  tc_fence_before();
-  __syncthreads();
-  if( warp == 0 ) asm volatile( "tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"( tmem ), "r"( (uint32_t) TC_TMEM_COLS ) : "memory" );
 }
 
 template<int N> static inline size_t trquant_tc_smem()
