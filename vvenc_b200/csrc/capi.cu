@@ -822,24 +822,25 @@ template<int LV>
 static int pyramidV2LaunchLevel( vvb_ctx* ctx, int orgPlane, int refPlane, const PyrLevels& lv, int rootFirst, int nRoots, int nx, int ny, const MePar& mp )
 {
   const PyrSmem L = pyr_smem<LV>( nx, ny );
-  const int NQ = ( 1 << ( 2 * ( LV - 1 ) ) ) / 4;
-  const int items = NQ * ( ( ny + 1 ) / 2 ) * L.nStrips;
-  // CTA size: one CTA per SM, so resident warps = CTA warps; measured on the 64x64 roots of the bench (4752 items): 640 threads 2.01 ms, 608 2.04, 512 2.02,
-  // 480 2.09, 448 2.26 -- more warps win over fewer idle slots in the last round.  Small roots / ranges: fewest idle thread slots, ties -> more threads.
-  int bd = PYR_MAX_THREADS;
-  if( items < 4 * PYR_MAX_THREADS )
+  const int NQ = ( 1 << ( 2 * ( LV - 1 ) ) ) / 4, maxT = pyr_max_threads<LV>();
+  const int items = NQ * ( ( ny + 1 ) / 2 ) * ( nx >> 3 ) + NQ * ( nx & 7 ) * ( ( ny + 7 ) / 8 );      // the kernel's strip items + column items
+  // CTA size: big grids take the largest CTA the instantiation allows (pyr_max_threads).  Small roots / ranges: fewest rounds of items per CTA (a CTA's rounds
+  // run one after another, and a grid of fewer roots than SMs takes as long as one CTA), then fewest idle thread slots, ties -> more threads.
+  int bd = maxT;
+  if( items < 4 * maxT )
   {
+    const int minRounds = ( items + maxT - 1 ) / maxT;
     double bestEff = -1.0;
-    for( int cand = 128; cand <= PYR_MAX_THREADS; cand += 32 )
+    for( int cand = 128; cand <= maxT; cand += 32 )
     {
       const int rounds = ( items + cand - 1 ) / cand;
       const double eff = (double) items / ( (double) rounds * cand );
-      if( eff >= bestEff - 1e-9 ) { bestEff = std::max( bestEff, eff ); bd = cand; }
+      if( rounds == minRounds && eff >= bestEff - 1e-9 ) { bestEff = std::max( bestEff, eff ); bd = cand; }
     }
   }
   static const int forced = []{ const char* e = getenv( "VVB_PYR_THREADS" ); return e ? atoi( e ) : 0; }();     // tuning aid: fixed CTA size
-  if( forced >= 64 && forced <= PYR_MAX_THREADS && ( forced & 31 ) == 0 ) bd = forced;
-  sad_pyramid8_kernel<LV><<<nRoots, bd, (size_t) L.total, ctx->stream>>>( ctx->planes.p[orgPlane], ctx->planes.p[refPlane], lv, rootFirst, nx, ny, mp, 1u, 8u );
+  if( forced >= 64 && forced <= maxT && ( forced & 31 ) == 0 ) bd = forced;
+  sad_pyramid8_kernel<LV><<<nRoots, bd, (size_t) L.total, ctx->stream>>>( ctx->planes.p[orgPlane], ctx->planes.p[refPlane], lv, rootFirst, nx, ny, mp, L, 1u, 8u );
   CHECK_LAUNCH( "sad_pyramid8_kernel" );
   return VVB_OK;
 }

@@ -14,15 +14,21 @@
 //   * odd-offset candidates read a second, one-pel-shifted copy of the window (no funnel shifts),
 //   * a thread evaluates TWO vertically adjacent candidate rows for a strip of 8 vectors: the nine window rows they need are loaded once (LDS.128) and
 //     every original row serves both (shared-memory traffic per candidate halves),
-//   * the epilogue per candidate is IDP.4A (MV bits of column + row -> table offset), LDS (rate table pre-multiplied by 8, one table per strip slot so
-//     that the slot index is part of the entry), IDP.2A (unpack the box sum and add it), IMAD (parent sum), IMAD (key) on the fma pipe and one VIMNMX.
+//   * the epilogue per candidate is IDP.4A (shared address of the rate entry: table base + row bits, plus column bits), LDS (rate table pre-multiplied
+//     by 8, one table per strip slot so that the slot index is part of the entry), IDP.2A (unpack the box sum and add it), IMAD (parent sum), IMAD (key)
+//     on the fma pipe and half a VIMNMX3.
 //   * strip slots past the end of the range carry MV-bit count 250 and read rate-table entries that can never win; no predicate per candidate.
+//   * the item keeps its base addresses and the four members step through fixed offsets.  For 32x32 and 64x64 roots the CTA has at most 512 threads so
+//     that ptxas may keep them in 128 registers (at 640 threads the 96-register cap forced their recomputation in every member).
 #pragma once
 #include "search_kernels.cuh"
 
 namespace vvb {
 
-#define PYR_MAX_THREADS 640
+// CTA size bound per root size.  A 64x64 root fills an SM's shared memory on its own; 512 threads leave 128 registers for the item loop.  16x16 roots need
+// about 64 KB, so several CTAs share an SM and registers set how many: the 640-thread bound (96 registers) lets two CTAs of the 320 threads that a
+// +-32 range picks run on one SM, where 120 registers would allow only one.
+template<int LV> constexpr int pyr_max_threads() { return LV == 2 ? 640 : 512; }
 #define PYR_MVN         296                      // rate-table entries per strip slot: 0..79 real, the rest "never wins" (padded columns index 250 + row bits)
 #define PYR_PAD_BITS    250
 #define PYR_NEVER       ( 1u << 26 )             // cost no real candidate reaches; 4 * PYR_NEVER * 8 still fits 32 bits
@@ -55,7 +61,7 @@ __host__ __device__ inline PyrSmem pyr_smem( int nx, int ny )
   s.vPitch  = R - 8 + s.nxp;
   s.nT      = LV == 4 ? 4 : ( LV == 3 ? 1 : 0 );
   s.tStride = ny * s.nxp;
-  // fixed-size tables first: their shared-memory addresses are then link-time constants (the rate look-up becomes LDS [reg + imm])
+  // fixed-size tables first: their offsets do not depend on the range
   int o = 0;
   s.offMv8  = o;   o += 8 * PYR_MVN * 4;
   s.offMvRaw = o;  o += VVB_MVCOST_ENTRIES * 4;
@@ -76,9 +82,13 @@ __host__ __device__ inline PyrSmem pyr_smem( int nx, int ny )
 
 __device__ __forceinline__ int pyr_compact( int v ) { v &= 0x55555555; v = ( v | ( v >> 1 ) ) & 0x33333333; v = ( v | ( v >> 2 ) ) & 0x0f0f0f0f; return ( v | ( v >> 4 ) ) & 0xff; }
 
-// one candidate row of one member: box sum + MV rate -> 8 packed (cost * 8 + slot) keys, running minimum; the SAD goes into the parent's sum
-__device__ __forceinline__ uint32_t pyr_finish_row( const int (&acc)[8], const uint16_t* __restrict__ vrow, uint2 bw, uint32_t by4, const unsigned char* __restrict__ mv8,
-                                                    uint32_t one, uint32_t eight, uint32_t (&ps)[8] )
+// rate-table entry at a 32-bit shared-memory address: the table base rides in the IDP.4A accumulator and the slot offset becomes the LDS immediate
+__device__ __forceinline__ uint32_t pyr_lds( uint32_t addr ) { uint32_t v; asm volatile( "ld.shared.u32 %0, [%1];" : "=r"( v ) : "r"( addr ) ); return v; }
+
+// one candidate row of one member: box sum + MV rate -> 8 packed (cost * 8 + slot) keys, running minimum; the SAD goes into the parent's sum.
+// mvRow = shared address of the rate tables + 4 * row bits
+__device__ __forceinline__ uint32_t pyr_finish_row( const int (&acc)[8], const uint16_t* __restrict__ vrow, uint2 bw, uint32_t mvRow, uint32_t one, uint32_t eight,
+                                                    uint32_t (&ps)[8] )
 {
   const uint4 vw = *reinterpret_cast<const uint4*>( vrow );
   const uint32_t v[4] = { vw.x, vw.y, vw.z, vw.w };
@@ -86,8 +96,8 @@ __device__ __forceinline__ uint32_t pyr_finish_row( const int (&acc)[8], const u
 #pragma unroll
   for( int k = 0; k < 8; k++ )
   {
-    const uint32_t idx4 = __dp4a( k < 4 ? bw.x : bw.y, 4u << ( 8 * ( k & 3 ) ), by4 );                  // 4 * (column bits + row bits)
-    const uint32_t mvk  = *reinterpret_cast<const uint32_t*>( mv8 + k * ( PYR_MVN * 4 ) + idx4 );        // rate * 8 + k
+    const uint32_t a    = __dp4a( k < 4 ? bw.x : bw.y, 4u << ( 8 * ( k & 3 ) ), mvRow );                  // + 4 * column bits
+    const uint32_t mvk  = pyr_lds( a + k * ( PYR_MVN * 4 ) );                                             // rate * 8 + k
     const uint32_t sad  = __dp2a_lo( v[k >> 1], ( k & 1 ) ? 0x0100u : 0x0001u, (uint32_t) acc[k] );      // box sum + (sum a - 2 sum min)
     ps[k] = sad * one + ps[k];                                                                             // IMAD: keeps the add off the alu pipe
     const uint32_t key = sad * eight + mvk;
@@ -97,14 +107,14 @@ __device__ __forceinline__ uint32_t pyr_finish_row( const int (&acc)[8], const u
 }
 
 template<int LV>
-__global__ void __launch_bounds__( PYR_MAX_THREADS, 1 ) sad_pyramid8_kernel( const __grid_constant__ Plane orgPlane, const __grid_constant__ Plane refPlane,
+__global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kernel( const __grid_constant__ Plane orgPlane, const __grid_constant__ Plane refPlane,
                                                                              const __grid_constant__ PyrLevels lv, int rootFirst, int nx, int ny,
-                                                                             const __grid_constant__ MePar par, uint32_t one, uint32_t eight )
+                                                                             const __grid_constant__ MePar par, const __grid_constant__ PyrSmem L,   // L = pyr_smem<LV>( nx, ny )
+                                                                             uint32_t one, uint32_t eight )
 {
   constexpr int R = 8 << ( LV - 1 ), NB0 = 1 << ( 2 * ( LV - 1 ) ), NQ = NB0 / 4, NBLK = ( 4 * NB0 - 1 ) / 3, LTOP = LV - 1;
-  constexpr int OFF1 = NB0, OFF2 = NB0 + NQ, OFF3 = NB0 + NQ + NQ / 4;
+  constexpr int OFF1 = NB0, OFF2 = NB0 + NQ, OFF3 = NB0 + NQ + NQ / 4, NT = LV == 4 ? 4 : ( LV == 3 ? 1 : 0 );
   extern __shared__ __align__( 128 ) unsigned char smemRaw[];
-  const PyrSmem L = pyr_smem<LV>( nx, ny );
   uint32_t* win0w = reinterpret_cast<uint32_t*>( smemRaw + L.offWin0 );
   uint32_t* win1w = reinterpret_cast<uint32_t*>( smemRaw + L.offWin1 );
   uint16_t* V     = reinterpret_cast<uint16_t*>( smemRaw + L.offV );
@@ -253,9 +263,10 @@ __global__ void __launch_bounds__( PYR_MAX_THREADS, 1 ) sad_pyramid8_kernel( con
       }
       *reinterpret_cast<uint4*>( Hs + r * L.vPitch + st * 8 ) = make_uint4( o[0], o[1], o[2], o[3] );
     }
+    const float invB = 1.0f / (float) L.bStride;
     for( int t = tid; t < NBLK * L.bStride; t += nthr )
     {
-      const int bid = t / L.bStride, e = t - bid * L.bStride;
+      const int bid = fast_div( t, invB ), e = t - bid * L.bStride;
       const int2 pr = sPred[bid];
       unsigned char v;
       if( e < nxp ) v = e < nx ? (unsigned char) eg_bits( ( ( rb.left + e ) * ( 1 << par.costScale ) - pr.x ) >> par.imvShift ) : (unsigned char) PYR_PAD_BITS;
@@ -283,136 +294,143 @@ __global__ void __launch_bounds__( PYR_MAX_THREADS, 1 ) sad_pyramid8_kernel( con
   if( LV >= 3 ) { for( int i = tid; i < L.nT * L.tStride; i += nthr ) T[i] = 0u; }
   __syncthreads();
 
-  // ---- candidates: item = (quad of four 8x8 members, pair of candidate rows, strip of 8 vectors)
+  // ---- candidates.  Strip item = (quad of four 8x8 members, pair of candidate rows, strip of 8 vectors); column item = (quad, one of the nx % 8 rightmost
+  // columns, group of 8 vertically adjacent vectors).  Both kinds share one item space, so the column items run in the short last round of the strip items
+  // instead of a round of their own.
   {
     // Lane mapping.  A quarter warp's LDS.128 is one wavefront when its 8 lanes read 8 consecutive 16-byte chunks: main items are groups of 8 adjacent strips
     // of one row pair (it = ((q * nPairs + pr) * nMain + st), st fastest); the strips left over when the range is not a multiple of 64 vectors follow as
     // tail items with the row pair as the fast index.
-    const int nFull = nx >> 3, nCols = nx & 7;                // full strips of 8 vectors; the nx % 8 columns left of them are column items (below)
+    const int nFull = nx >> 3, nCols = nx & 7;                // full strips of 8 vectors; the nx % 8 columns left of them are column items
     const int nPairs = ( ny + 1 ) >> 1, nMain = nFull & ~7, nTail = nFull - nMain;
-    const int perQm = nPairs * nMain, itemsMain = NQ * perQm, perQt = nPairs * nTail, items = itemsMain + NQ * perQt;
+    const int perQm = nPairs * nMain, itemsMain = NQ * perQm, perQt = nPairs * nTail, itemsStrip = itemsMain + NQ * perQt;
+    const int nV = ( ny + 7 ) >> 3, perQc = nCols * nV, items = itemsStrip + NQ * perQc;
     const float invPerQm = 1.0f / (float) max( 1, perQm ), invMain = 1.0f / (float) max( 1, nMain ), invPerQt = 1.0f / (float) max( 1, perQt ), invPairs = 1.0f / (float) nPairs;
+    const float invPerQc = 1.0f / (float) max( 1, perQc ), invNv = 1.0f / (float) nV;
     const uint32_t* org32 = reinterpret_cast<const uint32_t*>( orgS );
+    const uint32_t mvBase = (uint32_t) __cvta_generic_to_shared( sMv8 );
+    const int vPitch = L.vPitch, bStride = L.bStride;
     for( int base = 0; base < items; base += nthr )
     {
       const int it = base + tid;
-      const bool active = it < items;
-      const unsigned mask = __ballot_sync( 0xffffffffu, active );
-      if( !active ) continue;
-      int q, pr, st;
-      if( it < itemsMain ) { q = fast_div( it, invPerQm ); const int rem = it - q * perQm; pr = fast_div( rem, invMain ); st = rem - pr * nMain; }
-      else { const int i2 = it - itemsMain; q = fast_div( i2, invPerQt ); const int rem = i2 - q * perQt; const int ts = fast_div( rem, invPairs ); pr = rem - ts * nPairs; st = nMain + ts; }
-      const int cy = 2 * pr, cx0 = 8 * st;
-      const bool validB = cy + 1 < ny;
-      const int lead = __ffs( mask ) - 1;
-      const bool uni = __all_sync( mask, q == __shfl_sync( mask, q, lead ) );
-      const int qx = pyr_compact( q ), qy = pyr_compact( q >> 1 );
-      uint32_t psA[8], psB[8];
-#pragma unroll
-      for( int k = 0; k < 8; k++ ) { psA[k] = 0u; psB[k] = 0u; }
-#pragma unroll 1
-      for( int m = 0; m < 4; m++ )
+      const bool isStrip = it < itemsStrip, isCol = !isStrip && it < items;
+      const unsigned maskS = __ballot_sync( 0xffffffffu, isStrip ), maskC = __ballot_sync( 0xffffffffu, isCol );
+      if( isStrip )
       {
-        const int bx8 = 2 * qx + ( m & 1 ), by8 = 2 * qy + ( m >> 1 ), b0 = 4 * q + m;
-        const int sumA = sSumA[b0];
-        int accA[8], accB[8];
+        const unsigned mask = maskS;
+        int q, pr, st;
+        if( it < itemsMain ) { q = fast_div( it, invPerQm ); const int rem = it - q * perQm; pr = fast_div( rem, invMain ); st = rem - pr * nMain; }
+        else { const int i2 = it - itemsMain; q = fast_div( i2, invPerQt ); const int rem = i2 - q * perQt; const int ts = fast_div( rem, invPairs ); pr = rem - ts * nPairs; st = nMain + ts; }
+        const int cy = 2 * pr, cx0 = 8 * st;
+        const bool validB = cy + 1 < ny;
+        const int lead = __ffs( mask ) - 1;
+        const bool uni = __all_sync( mask, q == __shfl_sync( mask, q, lead ) );
+        const int qx = ( q & 1 ) | ( ( q >> 1 ) & 2 ), qy = ( ( q >> 1 ) & 1 ) | ( ( q >> 2 ) & 2 );     // z-order position of the quad (q < 16)
+        uint32_t psA[8], psB[8];
 #pragma unroll
-        for( int k = 0; k < 8; k++ ) { accA[k] = sumA; accB[k] = sumA; }
-        const uint32_t* op = org32 + ( by8 * 8 ) * ( R / 2 ) + bx8 * 4;
-        const int wofs = ( by8 * 8 + cy ) * wsw + bx8 * 4 + ( cx0 >> 1 );
+        for( int k = 0; k < 8; k++ ) { psA[k] = 0u; psB[k] = 0u; }
+        // member 0 of the quad; member m lies (m & 1) * 8 pels right and (m >> 1) * 8 rows down of it in the originals, the window and V
+        const uint32_t* op = org32 + ( qy * 16 ) * ( R / 2 ) + qx * 8;
+        const int wofs = ( qy * 16 + cy ) * wsw + qx * 8 + ( cx0 >> 1 );
         const uint32_t* w0 = win0w + wofs;
         const uint32_t* w1 = win1w + wofs;
-        uint4 oPrev = make_uint4( 0, 0, 0, 0 );
-#pragma unroll
-        for( int y = 0; y < 9; y++ )
+        const uint16_t* vrow = V + ( qy * 16 + cy ) * vPitch + qx * 16 + cx0;
+        const unsigned char* bb = bitsS + 4 * q * bStride;
+#pragma unroll 1
+        for( int m = 0; m < 4; m++ )
         {
-          const uint4 e0 = *reinterpret_cast<const uint4*>( w0 + y * wsw ), e1 = *reinterpret_cast<const uint4*>( w0 + y * wsw + 4 );
-          const uint4 d0 = *reinterpret_cast<const uint4*>( w1 + y * wsw ), d1 = *reinterpret_cast<const uint4*>( w1 + y * wsw + 4 );
-          const uint32_t e[8] = { e0.x, e0.y, e0.z, e0.w, e1.x, e1.y, e1.z, e1.w };
-          const uint32_t d[8] = { d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w };
-          uint4 oCur = oPrev;
-          if( y < 8 )
+          const int b0 = 4 * q + m;
+          const int sumA = sSumA[b0];
+          int accA[8], accB[8];
+#pragma unroll
+          for( int k = 0; k < 8; k++ ) { accA[k] = sumA; accB[k] = sumA; }
+          uint4 oPrev = make_uint4( 0, 0, 0, 0 );
+#pragma unroll
+          for( int y = 0; y < 9; y++ )
           {
-            oCur = *reinterpret_cast<const uint4*>( op + y * ( R / 2 ) );
-            const uint32_t o[4] = { oCur.x, oCur.y, oCur.z, oCur.w };
+            const uint4 e0 = *reinterpret_cast<const uint4*>( w0 + y * wsw ), e1 = *reinterpret_cast<const uint4*>( w0 + y * wsw + 4 );
+            const uint4 d0 = *reinterpret_cast<const uint4*>( w1 + y * wsw ), d1 = *reinterpret_cast<const uint4*>( w1 + y * wsw + 4 );
+            const uint32_t e[8] = { e0.x, e0.y, e0.z, e0.w, e1.x, e1.y, e1.z, e1.w };
+            const uint32_t d[8] = { d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w };
+            uint4 oCur = oPrev;
+            if( y < 8 )
+            {
+              oCur = *reinterpret_cast<const uint4*>( op + y * ( R / 2 ) );
+              const uint32_t o[4] = { oCur.x, oCur.y, oCur.z, oCur.w };
+#pragma unroll
+              for( int k = 0; k < 8; k++ )
+#pragma unroll
+                for( int i = 0; i < 4; i++ )
+                  accA[k] = __dp2a_lo( (int) __vmins2( o[i], ( k & 1 ) ? d[i + ( k >> 1 )] : e[i + ( k >> 1 )] ), (int) 0x0000fefeu, accA[k] );
+            }
+            if( y > 0 )
+            {
+              const uint32_t o[4] = { oPrev.x, oPrev.y, oPrev.z, oPrev.w };
+#pragma unroll
+              for( int k = 0; k < 8; k++ )
+#pragma unroll
+                for( int i = 0; i < 4; i++ )
+                  accB[k] = __dp2a_lo( (int) __vmins2( o[i], ( k & 1 ) ? d[i + ( k >> 1 )] : e[i + ( k >> 1 )] ), (int) 0x0000fefeu, accB[k] );
+            }
+            oPrev = oCur;
+          }
+          // member epilogue
+          const uint2 bw = *reinterpret_cast<const uint2*>( bb + cx0 );
+          uint32_t bk = pyr_finish_row( accA, vrow, bw, mvBase + bb[nxp + cy], one, eight, psA );
+          uint32_t key = ( ( bk >> 3 ) << ob ) + (uint32_t)( cy * nx + cx0 ) + ( bk & 7u );
+          if( validB )
+          {
+            bk = pyr_finish_row( accB, vrow + vPitch, bw, mvBase + bb[nxp + cy + 1], one, eight, psB );
+            key = min( key, ( ( bk >> 3 ) << ob ) + (uint32_t)( ( cy + 1 ) * nx + cx0 ) + ( bk & 7u ) );
+          }
+          if( uni ) { key = __reduce_min_sync( mask, key ); if( lane == lead ) atomicMin( &sKey32[b0], key ); }
+          else atomicMin( &sKey32[b0], key );
+          const bool right = !( m & 1 );                        // next member: one to the right, or back left and one down
+          op   += right ? 4 : 8 * ( R / 2 ) - 4;
+          w0   += right ? 4 : 8 * wsw - 4;
+          w1   += right ? 4 : 8 * wsw - 4;
+          vrow += right ? 8 : 8 * vPitch - 8;
+          bb   += bStride;
+        }
+        // the 16x16 parent of the quad: its SAD at a vector is the sum of the members' SADs
+        {
+          const unsigned char* pb = bitsS + ( OFF1 + q ) * bStride;
+          const uint2 bw = *reinterpret_cast<const uint2*>( pb + cx0 );
+          uint32_t* trow = LV >= 3 ? T + ( LV == 4 ? ( q >> 2 ) : 0 ) * L.tStride + cy * nxp + st : nullptr;      // table layout [cy][slot k][strip]: a warp's atomics spread over the banks
+          uint32_t key = 0xffffffffu;
+#pragma unroll
+          for( int rowB = 0; rowB < 2; rowB++ )
+          {
+            if( rowB && !validB ) break;
+            const uint32_t mvRow = mvBase + pb[nxp + cy + rowB];
+            uint32_t bk = 0xffffffffu;
 #pragma unroll
             for( int k = 0; k < 8; k++ )
-#pragma unroll
-              for( int i = 0; i < 4; i++ )
-                accA[k] = __dp2a_lo( (int) __vmins2( o[i], ( k & 1 ) ? d[i + ( k >> 1 )] : e[i + ( k >> 1 )] ), (int) 0x0000fefeu, accA[k] );
+            {
+              const uint32_t ps  = rowB ? psB[k] : psA[k];
+              const uint32_t a   = __dp4a( k < 4 ? bw.x : bw.y, 4u << ( 8 * ( k & 3 ) ), mvRow );
+              const uint32_t mvk = pyr_lds( a + k * ( PYR_MVN * 4 ) );
+              bk = min( bk, ps * eight + mvk );
+              if( LV >= 3 ) atomicAdd( trow + rowB * nxp + k * nStrips, ps );
+            }
+            key = min( key, ( ( bk >> 3 ) << ob ) + (uint32_t)( ( cy + rowB ) * nx + cx0 ) + ( bk & 7u ) );
           }
-          if( y > 0 )
-          {
-            const uint32_t o[4] = { oPrev.x, oPrev.y, oPrev.z, oPrev.w };
-#pragma unroll
-            for( int k = 0; k < 8; k++ )
-#pragma unroll
-              for( int i = 0; i < 4; i++ )
-                accB[k] = __dp2a_lo( (int) __vmins2( o[i], ( k & 1 ) ? d[i + ( k >> 1 )] : e[i + ( k >> 1 )] ), (int) 0x0000fefeu, accB[k] );
-          }
-          oPrev = oCur;
+          if( uni ) { key = __reduce_min_sync( mask, key ); if( lane == lead ) atomicMin( &sKey32[OFF1 + q], key ); }
+          else atomicMin( &sKey32[OFF1 + q], key );
         }
-        // member epilogue
-        const unsigned char* bb = bitsS + b0 * L.bStride;
-        const uint2 bw = *reinterpret_cast<const uint2*>( bb + cx0 );
-        const uint16_t* vrow = V + ( by8 * 8 + cy ) * L.vPitch + bx8 * 8 + cx0;
-        uint32_t bk = pyr_finish_row( accA, vrow, bw, bb[nxp + cy], sMv8, one, eight, psA );
-        uint32_t key = ( ( bk >> 3 ) << ob ) + (uint32_t)( cy * nx + cx0 ) + ( bk & 7u );
-        if( validB )
-        {
-          bk = pyr_finish_row( accB, vrow + L.vPitch, bw, bb[nxp + cy + 1], sMv8, one, eight, psB );
-          key = min( key, ( ( bk >> 3 ) << ob ) + (uint32_t)( ( cy + 1 ) * nx + cx0 ) + ( bk & 7u ) );
-        }
-        if( uni ) { key = __reduce_min_sync( mask, key ); if( lane == lead ) atomicMin( &sKey32[b0], key ); }
-        else atomicMin( &sKey32[b0], key );
       }
-      // the 16x16 parent of the quad: its SAD at a vector is the sum of the members' SADs
+      else if( isCol )
       {
-        const unsigned char* bb = bitsS + ( OFF1 + q ) * L.bStride;
-        const uint2 bw = *reinterpret_cast<const uint2*>( bb + cx0 );
-        uint32_t* trow = LV >= 3 ? T + ( LV == 4 ? ( q >> 2 ) : 0 ) * L.tStride + cy * nxp + st : nullptr;      // table layout [cy][slot k][strip]: a warp's atomics spread over the banks
-        uint32_t key = 0xffffffffu;
-#pragma unroll
-        for( int rowB = 0; rowB < 2; rowB++ )
-        {
-          if( rowB && !validB ) break;
-          const uint32_t by4 = bb[nxp + cy + rowB];
-          uint32_t bk = 0xffffffffu;
-#pragma unroll
-          for( int k = 0; k < 8; k++ )
-          {
-            const uint32_t ps = rowB ? psB[k] : psA[k];
-            const uint32_t idx4 = __dp4a( k < 4 ? bw.x : bw.y, 4u << ( 8 * ( k & 3 ) ), by4 );
-            const uint32_t mvk  = *reinterpret_cast<const uint32_t*>( sMv8 + k * ( PYR_MVN * 4 ) + idx4 );
-            bk = min( bk, ps * eight + mvk );
-            if( LV >= 3 ) atomicAdd( trow + rowB * nxp + k * nStrips, ps );
-          }
-          key = min( key, ( ( bk >> 3 ) << ob ) + (uint32_t)( ( cy + rowB ) * nx + cx0 ) + ( bk & 7u ) );
-        }
-        if( uni ) { key = __reduce_min_sync( mask, key ); if( lane == lead ) atomicMin( &sKey32[OFF1 + q], key ); }
-        else atomicMin( &sKey32[OFF1 + q], key );
-      }
-    }
-
-    // ---- the nx % 8 rightmost columns (one column for every +-R range): item = (quad, column, group of 8 vertically adjacent vectors).  A strip item would
-    // spend a full strip of work on them (11 % of the kernel for 65 columns); here the thread keeps the member's eight original rows in registers and walks
-    // the 15 window rows its 8 vectors touch: window row r meets original row r - c for vector c.
-    if( nCols )
-    {
-      const int nV = ( ny + 7 ) >> 3, perQc = nCols * nV, itemsC = NQ * perQc;
-      const float invPerQc = 1.0f / (float) perQc, invNv = 1.0f / (float) nV;
-      for( int base = 0; base < itemsC; base += nthr )
-      {
-        const int it = base + tid;
-        const bool active = it < itemsC;
-        const unsigned mask = __ballot_sync( 0xffffffffu, active );
-        if( !active ) continue;
-        const int q = fast_div( it, invPerQc ), rem = it - q * perQc;
+        // A strip item would spend a full strip of work on one column; here the thread keeps the member's eight original rows in registers and walks the
+        // 15 window rows its 8 vectors touch: window row r meets original row r - c for vector c.
+        const unsigned mask = maskC;
+        const int ic = it - itemsStrip;
+        const int q = fast_div( ic, invPerQc ), rem = ic - q * perQc;
         const int ci = fast_div( rem, invNv ), g = rem - ci * nV;
         const int cx = 8 * nFull + ci, cy0 = 8 * g;
         const int lead = __ffs( mask ) - 1;
         const bool uni = __all_sync( mask, q == __shfl_sync( mask, q, lead ) );
-        const int qx = pyr_compact( q ), qy = pyr_compact( q >> 1 );
+        const int qx = ( q & 1 ) | ( ( q >> 1 ) & 2 ), qy = ( ( q >> 1 ) & 1 ) | ( ( q >> 2 ) & 2 );
         const uint32_t* wsrc = ( cx & 1 ) ? win1w : win0w;      // odd columns read the one-pel-shifted copy
         const int cw = cx >> 1;                                 // word offset of the column inside a window row
         uint32_t ps[8];
@@ -450,17 +468,17 @@ __global__ void __launch_bounds__( PYR_MAX_THREADS, 1 ) sad_pyramid8_kernel( con
               }
             }
           }
-          const unsigned char* bb = bitsS + b0 * L.bStride;
-          const uint32_t bx4 = 4u * bb[cx];
+          const unsigned char* bb = bitsS + b0 * bStride;
+          const uint32_t mvCol = mvBase + 4u * bb[cx];
           const uint2 byw = *reinterpret_cast<const uint2*>( bb + nxp + cy0 );
-          const uint16_t* vcol = V + ( by8 * 8 + cy0 ) * L.vPitch + bx8 * 8 + cx;
+          const uint16_t* vcol = V + ( by8 * 8 + cy0 ) * vPitch + bx8 * 8 + cx;
           uint32_t bk = 0xffffffffu;
 #pragma unroll
           for( int c = 0; c < 8; c++ )
           {
-            const uint32_t idx4 = __dp4a( c < 4 ? byw.x : byw.y, 1u << ( 8 * ( c & 3 ) ), bx4 );              // row bits are stored times 4
-            const uint32_t mvk  = *reinterpret_cast<const uint32_t*>( sMv8 + c * ( PYR_MVN * 4 ) + idx4 );
-            const uint32_t sad  = (uint32_t)( (int) vcol[c * L.vPitch] + acc[c] );
+            const uint32_t a   = __dp4a( c < 4 ? byw.x : byw.y, 1u << ( 8 * ( c & 3 ) ), mvCol );           // row bits are stored times 4
+            const uint32_t mvk = pyr_lds( a + c * ( PYR_MVN * 4 ) );
+            const uint32_t sad = (uint32_t)( (int) vcol[c * vPitch] + acc[c] );
             ps[c] += sad;
             const uint32_t key = cy0 + c < ny ? sad * eight + mvk : 0xffffffffu;
             bk = min( bk, key );
@@ -470,16 +488,16 @@ __global__ void __launch_bounds__( PYR_MAX_THREADS, 1 ) sad_pyramid8_kernel( con
           else atomicMin( &sKey32[b0], key );
         }
         {
-          const unsigned char* bb = bitsS + ( OFF1 + q ) * L.bStride;
-          const uint32_t bx4 = 4u * bb[cx];
+          const unsigned char* bb = bitsS + ( OFF1 + q ) * bStride;
+          const uint32_t mvCol = mvBase + 4u * bb[cx];
           const uint2 byw = *reinterpret_cast<const uint2*>( bb + nxp + cy0 );
           uint32_t* tcol = LV >= 3 ? T + ( LV == 4 ? ( q >> 2 ) : 0 ) * L.tStride + cy0 * nxp + ( cx & 7 ) * nStrips + ( cx >> 3 ) : nullptr;
           uint32_t bk = 0xffffffffu;
 #pragma unroll
           for( int c = 0; c < 8; c++ )
           {
-            const uint32_t idx4 = __dp4a( c < 4 ? byw.x : byw.y, 1u << ( 8 * ( c & 3 ) ), bx4 );
-            const uint32_t mvk  = *reinterpret_cast<const uint32_t*>( sMv8 + c * ( PYR_MVN * 4 ) + idx4 );
+            const uint32_t a   = __dp4a( c < 4 ? byw.x : byw.y, 1u << ( 8 * ( c & 3 ) ), mvCol );
+            const uint32_t mvk = pyr_lds( a + c * ( PYR_MVN * 4 ) );
             if( cy0 + c < ny )
             {
               bk = min( bk, ps[c] * eight + mvk );
@@ -495,31 +513,37 @@ __global__ void __launch_bounds__( PYR_MAX_THREADS, 1 ) sad_pyramid8_kernel( con
   }
   __syncthreads();
 
-  // ---- 32x32 blocks from their tables, 64x64 root from the sum of the four tables
+  // ---- 32x32 blocks from their tables and the 64x64 root from the sum of the four, in one pass: every table entry is read once
   if( LV >= 3 )
   {
-    const int nTop = L.nT + ( LV == 4 ? 1 : 0 );
+    constexpr int NTOP = LV == 4 ? NT + 1 : 1;
     const float invNx = 1.0f / (float) nx;
-    for( int j = 0; j < nTop; j++ )
+    unsigned long long best[NTOP];
+#pragma unroll
+    for( int j = 0; j < NTOP; j++ ) best[j] = ~0ull;
+    for( int o = tid; o < nx * ny; o += nthr )
     {
-      const bool isRoot64 = LV == 4 && j == L.nT;
-      const int bid = isRoot64 ? OFF3 : OFF2 + j;
-      const unsigned char* bb = bitsS + bid * L.bStride;
-      unsigned long long best = ~0ull;
-      for( int o = tid; o < nx * ny; o += nthr )
+      const int cy = fast_div( o, invNx ), cx = o - cy * nx;
+      const int ti = cy * nxp + ( cx & 7 ) * nStrips + ( cx >> 3 );
+      uint32_t sum = 0u;
+#pragma unroll
+      for( int j = 0; j < NTOP; j++ )
       {
-        const int cy = fast_div( o, invNx ), cx = o - cy * nx;
-        const int ti = cy * nxp + ( cx & 7 ) * nStrips + ( cx >> 3 );
         uint32_t s;
-        if( isRoot64 ) s = T[ti] + T[L.tStride + ti] + T[2 * L.tStride + ti] + T[3 * L.tStride + ti];
-        else           s = T[j * L.tStride + ti];
+        if( j < NT ) { s = T[j * L.tStride + ti]; sum += s; }
+        else         s = sum;
+        const unsigned char* bb = bitsS + ( j < NT ? OFF2 + j : OFF3 ) * L.bStride;
         const uint32_t bits = (uint32_t) bb[cx] + ( (uint32_t) bb[nxp + cy] >> 2 );
         const unsigned long long key = ( ( (unsigned long long) s + sMvRaw[bits < VVB_MVCOST_ENTRIES ? bits : VVB_MVCOST_ENTRIES - 1] ) << 16 ) | (unsigned) o;
-        best = key < best ? key : best;
+        best[j] = key < best[j] ? key : best[j];
       }
+    }
 #pragma unroll
-      for( int mm = 16; mm > 0; mm >>= 1 ) { const unsigned long long o2 = __shfl_xor_sync( 0xffffffffu, best, mm ); best = o2 < best ? o2 : best; }
-      if( lane == 0 && best != ~0ull ) atomicMin( &sKey64[j], best );
+    for( int j = 0; j < NTOP; j++ )
+    {
+#pragma unroll
+      for( int mm = 16; mm > 0; mm >>= 1 ) { const unsigned long long o2 = __shfl_xor_sync( 0xffffffffu, best[j], mm ); best[j] = o2 < best[j] ? o2 : best[j]; }
+      if( lane == 0 && best[j] != ~0ull ) atomicMin( &sKey64[j], best[j] );
     }
     __syncthreads();
   }
