@@ -69,6 +69,8 @@ __device__ __forceinline__ uint32_t eg_bits( int v )
 #define VVB_MVCOST_ENTRIES 80
 struct MvCostTable { uint32_t cost[VVB_MVCOST_ENTRIES]; };   // cost[bits] = Distortion( sqrt(lambda) * bits ), host-computed in IEEE double
 
+enum class ScratchArena { Host, Work };                      // the two scratch arenas of a context (vvb_ctx::d_scratch)
+
 } // namespace vvb
 
 // ---- host side -------------------------------------------------------------------------------------------------
@@ -101,11 +103,12 @@ struct vvb_ctx
   void*          dqShapes    = nullptr;     // host: vvbdq::DqShapeTables[25]
   int16_t*       d_mask      = nullptr;     // GEO weight masks (vvb_mask_upload)
   int            maskCount   = 0;
-  // grow-only scratch arenas (device + pinned host) used by the host-buffer entry points
   int            mctfMaxDim = 64;      // largest MCTF block dimension in device-resident candidate lists (vvb_mctf_hint)
   bool           async = false;        // host-buffer calls enqueue only; vvb_synchronize() completes them (vvb_set_async)
-  void*          d_scratch[8] = {};
-  size_t         d_scratchSize[8] = {};
-  void*          h_pinned = nullptr;
-  size_t         h_pinnedSize = 0;
+  // Grow-only device scratch, indexed by vvb::ScratchArena.  Growing an arena synchronises the stream and frees the old buffer, so whoever holds an arena
+  // must not call anything that takes the same one:
+  //  - Host: the buffers of one host-buffer entry point or single-block helper, for the duration of that call; its _dev twin never takes Host.
+  //  - Work: the temporaries of a _dev call.  A _dev call that holds Work never calls another entry point that takes Work.
+  void*          d_scratch[2] = {};
+  size_t         d_scratchSize[2] = {};
 };
