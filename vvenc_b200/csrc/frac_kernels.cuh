@@ -9,7 +9,7 @@
 //
 // One CTA per block.  The window (h + 8 rows) is staged once; the horizontally filtered rows of one horizontal offset at a time (all seven at once for
 // 8x8 blocks) are computed once (packed as row pairs, IDP.2A) and shared by the 7 vertical offsets; a lane owns one (vertical offset, 8x8 tile): it runs the vertical filter for its
-// tile (IDP.2A on row pairs), forms the 64 differences in registers and either sums |d| or runs the 64-point 2-D Hadamard there (as had8_pattern_kernel).
+// tile (IDP.2A on row pairs), forms the 64 differences in registers and either sums |d| or runs the 64-point 2-D Hadamard there (as had8_direct_kernel).
 #pragma once
 #include "common.cuh"
 #include "dist_kernels.cuh"
