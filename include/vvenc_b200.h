@@ -221,11 +221,10 @@ int vvb_fwd_trquant    ( vvb_ctx* ctx, const vvb_tu_par* par, const int16_t* res
                          int32_t* coef, int16_t* q, int32_t* abs_sum, int32_t* last_pos, uint8_t* need_rdoq );
 int vvb_fwd_trquant_dev( vvb_ctx* ctx, const vvb_tu_par* par, const int16_t* dev_resi, int n,
                          int32_t* dev_coef, int16_t* dev_q, int32_t* dev_abs_sum, int32_t* dev_last_pos, uint8_t* dev_need_rdoq );
-/* Transform engine of vvb_fwd_trquant*: 0 = CUDA-core IDP.2A kernels for every shape; 1 = wgmma (s8, byte planes split by the threads, register accumulators)
- * for the square 16/32/64 TUs; 2 = that engine at 64x64 only; 3 (default) = the raw-byte wgmma engine (the MMAs read the bytes of the int16 residual / int32
- * stage-1 values as u8 / s8 against zero-interleaved matrices, quantiser in registers) for square 8..64 TUs with the plain quantiser,
- * CUDA cores elsewhere.
- * All engines are bit-exact. */
+/* Transform engine of vvb_fwd_trquant*, vvb_inv_trquant* and vvb_tu_roundtrip*: 0 = CUDA-core IDP.2A kernels for every shape; any other value (default) = the
+ * raw-byte wgmma engines (the MMAs read the bytes of the int16 residual / int32 stage-1 values as u8 / s8 against zero-interleaved matrices, quantiser in
+ * registers) where they apply: square 8..64 TUs without LFNST or transform skip (forward: also without sign-bit hiding); CUDA cores elsewhere.
+ * Both settings are bit-exact. */
 int vvb_set_tensor_transform( vvb_ctx* ctx, int enable );
 /* Residual formed on the device: resi = org(x,y) - pred(x+start_x, y+start_y) for each TU position (PelBuf::subtract, IntraSearch.cpp:1328) */
 int vvb_fwd_trquant_planes    ( vvb_ctx* ctx, const vvb_tu_par* par, int org_plane, int pred_plane, const vvb_block* blocks, int n,

@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Component timing of the TU kernels on pools larger than L2: forward (wgmma / IDP.2A), inverse, fused round trip.
+"""Component timing of the TU kernels on pools larger than L2: forward (tensor engine on / off), inverse, fused round trip.
 usage: python tools/tu_bench.py [noise_amp [WxH ...]]   (GPU box)"""
 import ctypes, sys, os
 import numpy as np, torch
@@ -40,19 +40,11 @@ for (w, h) in shapes:
     d_sum = torch.empty(ntu, dtype=torch.int32, device='cuda'); d_last = torch.empty_like(d_sum); d_nr = torch.empty(ntu, dtype=torch.uint8, device='cuda')
     torch.cuda.synchronize()
     res = {}
-    for tens in (3, 1, 0):
+    for (name, tens) in (('fwd_tensor', 1), ('fwd_cudacore', 0)):
         eng.set_tensor_transform(tens)
-        res['fwd_tc%d' % tens] = tl(lambda: chk(lib.vvb_fwd_trquant_dev(eng.h, ctypes.byref(par), P_(d_r.data_ptr()), ntu, None, P_(d_q.data_ptr()), P_(d_sum.data_ptr()),
-                                                                     P_(d_last.data_ptr()), P_(d_nr.data_ptr()))))
-    if os.environ.get('TC2_SWEEP'):
-        eng.set_tensor_transform(3)
-        for st in (3, 1):
-            for ct in (4, 6, 8):
-                os.environ['VVB_TC2_CTAS'] = str(ct); os.environ['VVB_TC2_STREAM'] = str(st)
-                res['fwd_s%dc%d' % (st, ct)] = tl(lambda: chk(lib.vvb_fwd_trquant_dev(eng.h, ctypes.byref(par), P_(d_r.data_ptr()), ntu, None, P_(d_q.data_ptr()), P_(d_sum.data_ptr()),
-                                                                                     P_(d_last.data_ptr()), P_(d_nr.data_ptr()))))
-        os.environ.pop('VVB_TC2_CTAS'); os.environ.pop('VVB_TC2_STREAM')
-    eng.set_tensor_transform(3)
+        res[name] = tl(lambda: chk(lib.vvb_fwd_trquant_dev(eng.h, ctypes.byref(par), P_(d_r.data_ptr()), ntu, None, P_(d_q.data_ptr()), P_(d_sum.data_ptr()),
+                                                        P_(d_last.data_ptr()), P_(d_nr.data_ptr()))))
+    eng.set_tensor_transform(1)
     res['inv'] = tl(lambda: chk(lib.vvb_inv_trquant_dev(eng.h, ctypes.byref(par), P_(d_q.data_ptr()), ntu, P_(d_rc.data_ptr()))))
     res['roundtrip'] = tl(lambda: chk(lib.vvb_tu_roundtrip_dev(eng.h, ctypes.byref(par), P_(d_o.data_ptr()), P_(d_p.data_ptr()), ntu, P_(d_q.data_ptr()), P_(d_rc.data_ptr()),
                                                                P_(d_rs.data_ptr()), None)))

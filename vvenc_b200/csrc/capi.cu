@@ -12,7 +12,6 @@
 #include "search_kernels.cuh"
 #include "pyramid_kernels.cuh"
 #include "trquant_kernels.cuh"
-#include "trquant_tc_kernels.cuh"
 #include "trquant_tc2_kernels.cuh"
 #include "itrquant_kernels.cuh"
 #include "itrquant_tc_kernels.cuh"
@@ -330,8 +329,8 @@ int vvb_create( vvb_ctx** out, int device )
     return VVB_ERR_CUDA;
   }
   // dynamic shared memory limits above the 48 KB default
-#define VVB_TC2_SMEM( Nv ) smemLimit( fwd_trquant_tc2_kernel<Nv, 0>, Tc2Shape<Nv>::SMEM ), smemLimit( fwd_trquant_tc2_kernel<Nv, 1>, Tc2Shape<Nv>::SMEM ), \
-                           smemLimit( fwd_trquant_tc2_kernel<Nv, 2>, Tc2Shape<Nv>::SMEM )
+#define VVB_FWD_TC_SMEM( Nv ) smemLimit( fwd_trquant_tc2_kernel<Nv, 0>, Tc2Shape<Nv>::SMEM ), smemLimit( fwd_trquant_tc2_kernel<Nv, 1>, Tc2Shape<Nv>::SMEM ), \
+                              smemLimit( fwd_trquant_tc2_kernel<Nv, 2>, Tc2Shape<Nv>::SMEM )
 #define VVB_ITC_SMEM( Nv ) smemLimit( inv_trquant_tc_kernel<Nv, false>, ItcShape<Nv>::SMEM ), smemLimit( inv_trquant_tc_kernel<Nv, true>, ItcShape<Nv>::SMEM )
 #define VVB_RING_SMEM( W ) smemLimit( had8_ring_kernel<true, W, 2>, 220 * 1024 ), smemLimit( had8_ring_kernel<false, W, 2>, 220 * 1024 ), \
                            smemLimit( had8_ring_kernel<true, W, 8>, 220 * 1024 ), smemLimit( had8_ring_kernel<false, W, 8>, 220 * 1024 )
@@ -345,9 +344,8 @@ int vvb_create( vvb_ctx** out, int device )
     smemLimit( mctf_error_packed_kernel, 100 * 1024 ), smemLimit( mctf_grid_kernel, 200 * 1024 ), smemLimit( mctf_wave_kernel, 100 * 1024 ),
     smemLimit( mctf_int_grid_kernel, 100 * 1024 ), smemLimit( mctf_apply_kernel, 100 * 1024 ), smemLimit( frac_grid_kernel, 100 * 1024 ),
     smemLimit( frac_grid_generic_kernel, 100 * 1024 ),
-    VVB_TC2_SMEM( 8 ), VVB_TC2_SMEM( 16 ), VVB_TC2_SMEM( 32 ), VVB_TC2_SMEM( 64 ), VVB_ITC_SMEM( 8 ), VVB_ITC_SMEM( 16 ), VVB_ITC_SMEM( 32 ), VVB_ITC_SMEM( 64 ),
-    smemLimit( fwd_trquant_tc_kernel<16>, 100 * 1024 ), smemLimit( fwd_trquant_tc_kernel<32>, 100 * 1024 ), smemLimit( fwd_trquant_tc_kernel<64>, 100 * 1024 ) };
-#undef VVB_TC2_SMEM
+    VVB_FWD_TC_SMEM( 8 ), VVB_FWD_TC_SMEM( 16 ), VVB_FWD_TC_SMEM( 32 ), VVB_FWD_TC_SMEM( 64 ), VVB_ITC_SMEM( 8 ), VVB_ITC_SMEM( 16 ), VVB_ITC_SMEM( 32 ), VVB_ITC_SMEM( 64 ) };
+#undef VVB_FWD_TC_SMEM
 #undef VVB_ITC_SMEM
 #undef VVB_RING_SMEM
   for( const auto& s : smemLimits ) cudaFuncSetAttribute( s.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, s.bytes );
@@ -412,11 +410,11 @@ int vvb_set_pyramid_engine( vvb_ctx* ctx, int engine )
   return VVB_OK;
 }
 
-// selects the transform engine (include/vvenc_b200.h): 3 = raw-byte wgmma engine (default), 1 / 2 = byte-plane wgmma engine, 0 = IDP.2A CUDA-core kernels
+// transform engine (include/vvenc_b200.h): non-zero (default) = the raw-byte wgmma engines where they apply, 0 = IDP.2A CUDA-core kernels for every shape
 int vvb_set_tensor_transform( vvb_ctx* ctx, int enable )
 {
   if( !ctx ) return VVB_ERR_ARG;
-  ctx->tensorTransform = enable;
+  ctx->tensorTransform = enable != 0;
   return VVB_OK;
 }
 
@@ -913,6 +911,26 @@ static int hadRingLaunch( vvb_ctx* ctx, const Plane& op, const Plane& rp, const 
   return VVB_OK;
 }
 
+// B operand image of a tensor engine (table: vvb_ctx::tc2Image or itcImage) for the size and transform pair of p: build( std::integral_constant<int, N>, img )
+// fills it on the host at the first use, then it stays on the device
+template<class Build> static int bImage( vvb_ctx* ctx, const TuPar& p, void* ( &table )[36], const uint4** out, Build build )
+{
+  void*& slot = table[( ( p.lw - 3 ) * 3 + p.trHor ) * 3 + p.trVer];
+  if( !slot )
+  {
+    std::vector<unsigned char> img;
+    switch( p.w ) { case 8: build( std::integral_constant<int, 8>(), img ); break; case 16: build( std::integral_constant<int, 16>(), img ); break;
+                    case 32: build( std::integral_constant<int, 32>(), img ); break; default: build( std::integral_constant<int, 64>(), img ); break; }
+    void* d = nullptr;
+    CU( cudaMalloc( &d, img.size() ) );
+    CU( cudaMemcpyAsync( d, img.data(), img.size(), cudaMemcpyHostToDevice, ctx->stream ) );
+    CU( cudaStreamSynchronize( ctx->stream ) );                // img is a local
+    slot = d;
+  }
+  *out = (const uint4*) slot;
+  return VVB_OK;
+}
+
 extern "C" {
 
 // SAD pyramid (see include/vvenc_b200.h): pel work at the base level only, every higher level is the exact sum of its children's SADs
@@ -1187,46 +1205,33 @@ static int makeTuPar( vvb_ctx* ctx, const vvb_tu_par* in, TuPar& p )
   return VVB_OK;
 }
 
-// second tensor-core engine (trquant_tc2_kernels.cuh): square TUs 8..64 with the plain quantiser
+// forward tensor-core engine (trquant_tc2_kernels.cuh): square TUs 8..64 with the plain quantiser
 static bool tc2Eligible( const vvb_ctx* ctx, const TuPar& p )
 {
-  return ctx->tensorTransform == 3 && !p.lfnstIdx && !p.ts && !p.signHiding && p.w == p.h && p.w >= 8 && p.w <= 64 && p.s1 >= 0;
+  return ctx->tensorTransform && !p.lfnstIdx && !p.ts && !p.signHiding && p.w == p.h && p.w >= 8 && p.w <= 64 && p.s1 >= 0;
 }
 // dResi alone: residual pool; dResi + dResi2: original and prediction pools; dBlocks: positions in the two planes
 static int tc2Launch( vvb_ctx* ctx, const TuPar& p, const int16_t* dResi, int orgPlane, int predPlane, const vvb_block* dBlocks, int n,
                       int32_t* dCoef, int16_t* dQ, int32_t* dAbsSum, int32_t* dLastPos, uint8_t* dNeedRdoq, const int16_t* dResi2 = nullptr )
 {
   const Plane po = dBlocks ? ctx->planes.p[orgPlane] : Plane{}, pp = dBlocks ? ctx->planes.p[predPlane] : Plane{};
-  // B operand images, built once per (size, horizontal type, vertical type) and kept on the device
-  const int key = ( ( p.lw - 3 ) * 3 + p.trHor ) * 3 + p.trVer;
-  if( !ctx->tc2Image[key] )
-  {
-    std::vector<unsigned char> img;
-#define VVB_TC2_IMG( Nv ) { using S = Tc2Shape<Nv>; img.resize( 2 * S::B1_BYTES + 3 * S::B2_BYTES ); tc2_build_b_image<Nv>( vvc_tr_table_host, p.offH, p.offV, p.keepW, p.keepH, img.data() ); }
-    switch( p.w ) { case 8: VVB_TC2_IMG( 8 ) break; case 16: VVB_TC2_IMG( 16 ) break; case 32: VVB_TC2_IMG( 32 ) break; default: VVB_TC2_IMG( 64 ) break; }
-#undef VVB_TC2_IMG
-    void* d = nullptr;
-    CU( cudaMalloc( &d, img.size() ) );
-    CU( cudaMemcpyAsync( d, img.data(), img.size(), cudaMemcpyHostToDevice, ctx->stream ) );
-    CU( cudaStreamSynchronize( ctx->stream ) );                // img is a local
-    ctx->tc2Image[key] = d;
-  }
-  const uint4* dImg = (const uint4*) ctx->tc2Image[key];
-  const char* envC = getenv( "VVB_TC2_CTAS" ); const char* envS = getenv( "VVB_TC2_STREAM" );     // tuning knobs: CTAs per SM; bit 0 cp.async streaming
-  const int capC = envC ? atoi( envC ) : 0, streamOn = envS ? atoi( envS ) : 1;
-#define VVB_TC2_CALL( Nv ) { using S = Tc2Shape<Nv>; const int tiles = ( n + S::TPT - 1 ) / S::TPT; \
+  const uint4* dImg; int rc;
+  if( ( rc = bImage( ctx, p, ctx->tc2Image, &dImg, [&]( auto nc, std::vector<unsigned char>& img ) {
+          constexpr int N = decltype( nc )::value; using S = Tc2Shape<N>;
+          img.resize( 2 * S::B1_BYTES + 3 * S::B2_BYTES ); tc2_build_b_image<N>( vvc_tr_table_host, p.offH, p.offV, p.keepW, p.keepH, img.data() ); } ) ) ) return rc;
+#define VVB_FWD_TC_CALL( Nv ) { using S = Tc2Shape<Nv>; const int tiles = ( n + S::TPT - 1 ) / S::TPT; \
     static int perSm[3] = { 0, 0, 0 }; const int mode = dBlocks ? 1 : dResi2 ? 2 : 0; int& ps = perSm[mode]; \
     if( !ps ) { cudaFuncAttributes fa = {}; \
                 if( mode == 1 ) cudaFuncGetAttributes( &fa, fwd_trquant_tc2_kernel<Nv, 1> ); else if( mode == 2 ) cudaFuncGetAttributes( &fa, fwd_trquant_tc2_kernel<Nv, 2> ); \
                 else cudaFuncGetAttributes( &fa, fwd_trquant_tc2_kernel<Nv, 0> ); \
                 const int regs = std::max( fa.numRegs, 32 ); \
                 ps = std::min( 65536 / ( regs * 128 ), ( 227 * 1024 ) / ( (int) S::SMEM + (int) fa.sharedSizeBytes + 1024 ) ); ps = std::max( std::min( ps, Nv == 8 ? 6 : 8 ), 1 ); } \
-    const int grid = std::min( tiles, ctx->numSMs * ( capC > 0 ? std::min( capC, ps ) : ps ) ); \
-    if( mode == 1 )      fwd_trquant_tc2_kernel<Nv, 1><<<grid, 128, S::SMEM, ctx->stream>>>( p, dImg, streamOn, ctx->d_scan, nullptr, nullptr, po, pp, dBlocks, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq ); \
-    else if( mode == 2 ) fwd_trquant_tc2_kernel<Nv, 2><<<grid, 128, S::SMEM, ctx->stream>>>( p, dImg, streamOn, ctx->d_scan, dResi, dResi2, po, pp, nullptr, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq ); \
-    else                 fwd_trquant_tc2_kernel<Nv, 0><<<grid, 128, S::SMEM, ctx->stream>>>( p, dImg, streamOn, ctx->d_scan, dResi, nullptr, po, pp, nullptr, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq ); }
-  switch( p.w ) { case 8: VVB_TC2_CALL( 8 ) break; case 16: VVB_TC2_CALL( 16 ) break; case 32: VVB_TC2_CALL( 32 ) break; default: VVB_TC2_CALL( 64 ) break; }
-#undef VVB_TC2_CALL
+    const int grid = std::min( tiles, ctx->numSMs * ps ); \
+    if( mode == 1 )      fwd_trquant_tc2_kernel<Nv, 1><<<grid, 128, S::SMEM, ctx->stream>>>( p, dImg, ctx->d_scan, nullptr, nullptr, po, pp, dBlocks, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq ); \
+    else if( mode == 2 ) fwd_trquant_tc2_kernel<Nv, 2><<<grid, 128, S::SMEM, ctx->stream>>>( p, dImg, ctx->d_scan, dResi, dResi2, po, pp, nullptr, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq ); \
+    else                 fwd_trquant_tc2_kernel<Nv, 0><<<grid, 128, S::SMEM, ctx->stream>>>( p, dImg, ctx->d_scan, dResi, nullptr, po, pp, nullptr, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq ); }
+  switch( p.w ) { case 8: VVB_FWD_TC_CALL( 8 ) break; case 16: VVB_FWD_TC_CALL( 16 ) break; case 32: VVB_FWD_TC_CALL( 32 ) break; default: VVB_FWD_TC_CALL( 64 ) break; }
+#undef VVB_FWD_TC_CALL
   CHECK_LAUNCH( "fwd_trquant_tc2_kernel" );
   return VVB_OK;
 }
@@ -1234,26 +1239,16 @@ static int tc2Launch( vvb_ctx* ctx, const TuPar& p, const int16_t* dResi, int or
 // inverse tensor-core engine (itrquant_tc_kernels.cuh): square 8 / 16 / 32 TUs, plain or DepQuant dequantiser parameters in p, no LFNST / transform skip
 static bool itcEligible( const vvb_ctx* ctx, const TuPar& p, const void* dQ )
 {
-  return ctx->tensorTransform == 3 && !p.lfnstIdx && !p.ts && p.w == p.h && p.w >= 8 && p.w <= 64 && ( ( (uintptr_t) dQ ) & 15 ) == 0;
+  return ctx->tensorTransform && !p.lfnstIdx && !p.ts && p.w == p.h && p.w >= 8 && p.w <= 64 && ( ( (uintptr_t) dQ ) & 15 ) == 0;
 }
 // dResi != nullptr: levels -> residual.  Otherwise the second half of the TU round trip (reconstruction + distortions; dSum / dLast from the forward engine)
 static int itcLaunch( vvb_ctx* ctx, const TuPar& p, const int16_t* dQ, int n, int16_t* dResi,
                       int orgPlane, int predPlane, const vvb_block* dBlocks, const int16_t* dOrg, const int16_t* dPred, int16_t* dReco, TuResult* dRes, const int32_t* dSum, const int32_t* dLast )
 {
-  const int key = ( ( p.lw - 3 ) * 3 + p.trHor ) * 3 + p.trVer;
-  if( !ctx->itcImage[key] )
-  {
-    std::vector<unsigned char> img;
-#define VVB_ITC_IMG( Nv ) { using S = ItcShape<Nv>; img.resize( 4 * S::B_BYTES ); itc_build_b_image<Nv>( vvc_tr_table_host, p.offH, p.offV, p.keepW, p.keepH, img.data() ); }
-    switch( p.w ) { case 8: VVB_ITC_IMG( 8 ) break; case 16: VVB_ITC_IMG( 16 ) break; case 32: VVB_ITC_IMG( 32 ) break; default: VVB_ITC_IMG( 64 ) break; }
-#undef VVB_ITC_IMG
-    void* d = nullptr;
-    CU( cudaMalloc( &d, img.size() ) );
-    CU( cudaMemcpyAsync( d, img.data(), img.size(), cudaMemcpyHostToDevice, ctx->stream ) );
-    CU( cudaStreamSynchronize( ctx->stream ) );
-    ctx->itcImage[key] = d;
-  }
-  const uint4* dImg = (const uint4*) ctx->itcImage[key];
+  const uint4* dImg; int rc;
+  if( ( rc = bImage( ctx, p, ctx->itcImage, &dImg, [&]( auto nc, std::vector<unsigned char>& img ) {
+          constexpr int N = decltype( nc )::value;
+          img.resize( 4 * ItcShape<N>::B_BYTES ); itc_build_b_image<N>( vvc_tr_table_host, p.offH, p.offV, p.keepW, p.keepH, img.data() ); } ) ) ) return rc;
   const Plane po = dBlocks ? ctx->planes.p[orgPlane] : Plane{}, pp = dBlocks ? ctx->planes.p[predPlane] : Plane{};
 #define VVB_ITC_CALL( Nv ) { using S = ItcShape<Nv>; const int tiles = ( n + S::TPT - 1 ) / S::TPT; const int grid = std::min( tiles, ctx->numSMs * std::min( 6, ( 227 * 1024 ) / ( S::SMEM + 1024 ) ) ); \
     if( dResi ) inv_trquant_tc_kernel<Nv, false><<<grid, 128, S::SMEM, ctx->stream>>>( p, dImg, dQ, n, dResi, 0, po, pp, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr ); \
@@ -1273,18 +1268,6 @@ int vvb_fwd_trquant_dev( vvb_ctx* ctx, const vvb_tu_par* par, const int16_t* dRe
   if( n == 0 ) return VVB_OK;
   CU( cudaSetDevice( ctx->device ) );
   if( tc2Eligible( ctx, p ) ) return tc2Launch( ctx, p, dResi, 0, 0, nullptr, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq );
-  if( !p.lfnstIdx && !p.ts && p.w == p.h && ( ( ctx->tensorTransform == 1 && ( p.w == 16 || p.w == 32 || p.w == 64 ) ) || ( ctx->tensorTransform == 2 && p.w == 64 ) ) )
-  {
-    // byte-plane wgmma path: 128 stacked rows (128/N TUs) per tile, persistent CTAs
-    const int tpt = 128 / p.w;
-    const int tiles = ( n + tpt - 1 ) / tpt;
-    const int grid = std::min( tiles, ctx->numSMs * 3 );
-    if( p.w == 16 )      fwd_trquant_tc_kernel<16><<<grid, 128, trquant_tc_smem<16>(), ctx->stream>>>( p, ctx->d_trTable, ctx->d_scan, dResi, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq );
-    else if( p.w == 32 ) fwd_trquant_tc_kernel<32><<<grid, 128, trquant_tc_smem<32>(), ctx->stream>>>( p, ctx->d_trTable, ctx->d_scan, dResi, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq );
-    else                 fwd_trquant_tc_kernel<64><<<grid, 128, trquant_tc_smem<64>(), ctx->stream>>>( p, ctx->d_trTable, ctx->d_scan, dResi, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq );
-    CHECK_LAUNCH( "fwd_trquant_tc_kernel" );
-    return VVB_OK;
-  }
   const bool ext = p.lfnstIdx != 0 || p.signHiding != 0 || p.ts != 0;        // the plain instantiation carries neither the LFNST stage, the sign-bit hiding pass nor transform skip
 #define VVB_FWD_CALL( LWv, LHv ) { using S = TuShape<LWv, LHv>; const size_t smem = (size_t)( S::MAT_WORDS + S::NTEAMS * S::TEAM_WORDS ) * 4; \
     if( ext ) fwd_trquant_kernel<LWv, LHv, true><<<teamGrid( ctx, n, S::NTEAMS, smem ), 128, smem, ctx->stream>>>( p, ctx->d_trTable, ctx->d_scan, dResi, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq ); \
@@ -1312,34 +1295,20 @@ int vvb_fwd_trquant_planes_dev( vvb_ctx* ctx, const vvb_tu_par* par, int orgPlan
   if( !validPlane( ctx, orgPlane ) || !validPlane( ctx, predPlane ) ) return fail( ctx, VVB_ERR_ARG, "unknown plane" );
   if( n == 0 ) return VVB_OK;
   CU( cudaSetDevice( ctx->device ) );
-  int rc;
-  {
-    // CUDA-core engine: the residual is formed while the TU is loaded (one launch, no compact residual buffer); the byte-plane wgmma engine keeps the staging kernel
-    TuPar p;
-    if( ( rc = makeTuPar( ctx, par, p ) ) ) return rc;
-    if( tc2Eligible( ctx, p ) ) return tc2Launch( ctx, p, nullptr, orgPlane, predPlane, dBlocks, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq );
-    const bool tensor = !p.lfnstIdx && !p.ts && p.w == p.h && ( ( ctx->tensorTransform == 1 && ( p.w == 16 || p.w == 32 || p.w == 64 ) ) || ( ctx->tensorTransform == 2 && p.w == 64 ) );
-    if( !tensor )
-    {
-      const Plane &po = ctx->planes.p[orgPlane], &pp = ctx->planes.p[predPlane];
-      const bool ext = p.lfnstIdx != 0 || p.signHiding != 0 || p.ts != 0;
+  TuPar p;
+  int rc = makeTuPar( ctx, par, p );
+  if( rc ) return rc;
+  if( tc2Eligible( ctx, p ) ) return tc2Launch( ctx, p, nullptr, orgPlane, predPlane, dBlocks, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq );
+  // CUDA-core engine: the residual is formed while the TU is loaded (one launch, no compact residual buffer)
+  const Plane &po = ctx->planes.p[orgPlane], &pp = ctx->planes.p[predPlane];
+  const bool ext = p.lfnstIdx != 0 || p.signHiding != 0 || p.ts != 0;
 #define VVB_FWDP_CALL( LWv, LHv ) { using S = TuShape<LWv, LHv>; const size_t smem = (size_t)( S::MAT_WORDS + S::NTEAMS * S::TEAM_WORDS ) * 4; \
-      if( ext ) fwd_trquant_planes_kernel<LWv, LHv, true><<<teamGrid( ctx, n, S::NTEAMS, smem ), 128, smem, ctx->stream>>>( p, ctx->d_trTable, ctx->d_scan, po, pp, dBlocks, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq ); \
-      else      fwd_trquant_planes_kernel<LWv, LHv, false><<<teamGrid( ctx, n, S::NTEAMS, smem ), 128, smem, ctx->stream>>>( p, ctx->d_trTable, ctx->d_scan, po, pp, dBlocks, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq ); }
-      VVB_TU_DISPATCH( p.lw, p.lh, VVB_FWDP_CALL )
+    if( ext ) fwd_trquant_planes_kernel<LWv, LHv, true><<<teamGrid( ctx, n, S::NTEAMS, smem ), 128, smem, ctx->stream>>>( p, ctx->d_trTable, ctx->d_scan, po, pp, dBlocks, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq ); \
+    else      fwd_trquant_planes_kernel<LWv, LHv, false><<<teamGrid( ctx, n, S::NTEAMS, smem ), 128, smem, ctx->stream>>>( p, ctx->d_trTable, ctx->d_scan, po, pp, dBlocks, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq ); }
+  VVB_TU_DISPATCH( p.lw, p.lh, VVB_FWDP_CALL )
 #undef VVB_FWDP_CALL
-      CHECK_LAUNCH( "fwd_trquant_planes_kernel" );
-      return VVB_OK;
-    }
-  }
-  void* dR;
-  const size_t area = (size_t) par->w * par->h;
-  if( ( rc = scratch( ctx, ScratchArena::Work, (size_t) n * area * 2, &dR ) ) ) return rc;
-  const long long total = (long long) n * area;
-  const int grid = (int) std::min<long long>( ( total + 255 ) / 256, (long long) ctx->numSMs * 16 );
-  residual_from_planes_kernel<<<grid, 256, 0, ctx->stream>>>( ctx->planes.p[orgPlane], ctx->planes.p[predPlane], dBlocks, n, par->w, par->h, (int16_t*) dR );
-  CHECK_LAUNCH( "residual_from_planes_kernel" );
-  return vvb_fwd_trquant_dev( ctx, par, (const int16_t*) dR, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq );
+  CHECK_LAUNCH( "fwd_trquant_planes_kernel" );
+  return VVB_OK;
 }
 
 int vvb_fwd_trquant_planes( vvb_ctx* ctx, const vvb_tu_par* par, int orgPlane, int predPlane, const vvb_block* blocks, int n,

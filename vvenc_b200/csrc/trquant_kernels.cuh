@@ -581,21 +581,4 @@ __global__ void __launch_bounds__( 128 ) fwd_trquant_planes_kernel( const __grid
   switch( lw ) { case 2: VVB_TU_DISPATCH_LH( 2, lh, CALL ) break; case 3: VVB_TU_DISPATCH_LH( 3, lh, CALL ) break; case 4: VVB_TU_DISPATCH_LH( 4, lh, CALL ) break; \
                  case 5: VVB_TU_DISPATCH_LH( 5, lh, CALL ) break; default: VVB_TU_DISPATCH_LH( 6, lh, CALL ) break; }
 
-// residual = org(x,y) - pred(x + start_x, y + start_y), written compactly so that fwd_trquant_kernel can consume it
-__global__ void residual_from_planes_kernel( const __grid_constant__ Plane orgPlane, const __grid_constant__ Plane predPlane,
-                                             const vvb_block* __restrict__ blocks, int n, int w, int h, int16_t* __restrict__ resi )
-{
-  const int area = w * h;
-  const long long total = (long long) n * area;
-  for( long long i = (long long) blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long) gridDim.x * blockDim.x )
-  {
-    const int b = (int)( i / area ), r = (int)( i - (long long) b * area );
-    const int y = r / w, x = r - y * w;
-    const vvb_block blk = blocks[b];
-    const int o = __ldg( orgPlane.origin + (ptrdiff_t)( blk.y + y ) * orgPlane.stride + blk.x + x );
-    const int p = __ldg( predPlane.origin + (ptrdiff_t)( blk.y + blk.start_y + y ) * predPlane.stride + blk.x + blk.start_x + x );
-    resi[i] = (int16_t)( o - p );
-  }
-}
-
 } // namespace vvb

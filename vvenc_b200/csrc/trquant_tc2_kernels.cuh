@@ -1,7 +1,6 @@
-// trquant_tc2_kernels.cuh -- forward 2-D integer transform + quantiser of square TUs 8x8 .. 64x64 on the wgmma tensor cores, second engine.
+// trquant_tc2_kernels.cuh -- forward 2-D integer transform + quantiser of square TUs 8x8 .. 64x64 on the wgmma tensor cores.
 //
-// What changed against trquant_tc_kernels.cuh (kept as engine 1 / 2 for A/B runs): the operands of the MMAs are the RAW little-endian bytes of the
-// values, so no thread ever splits a number into planes:
+// The operands of the MMAs are the RAW little-endian bytes of the values, so no thread ever splits a number into planes:
 //   stage 1:  A1[row (tu, y)][2x + b] = byte b of the int16 residual r[y][x]            (a plain 16-byte copy of the residual row)
 //             B1lo[j][2x] = Th[j][x], B1lo[j][2x+1] = 0 ; B1hi[j][2x] = 0, B1hi[j][2x+1] = Th[j][x]
 //             Dlo = A1(u8) x B1lo^T , Dhi = A1(s8) x B1hi^T : sum_x r * Th[j][x] = Dlo + 256 * Dhi      (low byte unsigned, high byte signed)
@@ -20,7 +19,8 @@
 //      (last significant position, coefficient-group masks, sums), levels go out as int16 with 2*KEEP-byte row segments per warp store.
 // The quantiser restates team_quantise (trquant_kernels.cuh) for EXT = false: plain quantiser, no LFNST limit, no sign-bit hiding, no transform skip.
 #pragma once
-#include "trquant_tc_kernels.cuh"
+#include "wgmma.cuh"
+#include "trquant_kernels.cuh"
 
 namespace vvb {
 
@@ -109,7 +109,7 @@ template<int N> static void tc2_build_b_image( const int8_t* tab, int offH, int 
 
 // MODE 0: compact residual pool (resi); 1: residual formed from resident planes at the block positions; 2: residual = resi[] - resi2[] of two compact pools (org, pred)
 template<int N, int MODE>
-__global__ void __launch_bounds__( 128, N >= 32 ? 3 : 4 ) fwd_trquant_tc2_kernel( const __grid_constant__ TuPar par, const uint4* __restrict__ bImage, int streamOn, const int32_t* __restrict__ scanTab,
+__global__ void __launch_bounds__( 128, N >= 32 ? 3 : 4 ) fwd_trquant_tc2_kernel( const __grid_constant__ TuPar par, const uint4* __restrict__ bImage, const int32_t* __restrict__ scanTab,
                                                                     const int16_t* __restrict__ resi, const int16_t* __restrict__ resi2,
                                                                     const __grid_constant__ Plane orgPlane, const __grid_constant__ Plane predPlane, const vvb_block* __restrict__ blocks,
                                                                     int n, int32_t* __restrict__ coefOut, int16_t* __restrict__ qOut, int32_t* __restrict__ absSumOut,
@@ -149,8 +149,7 @@ __global__ void __launch_bounds__( 128, N >= 32 ? 3 : 4 ) fwd_trquant_tc2_kernel
   // ---- A: residual rows of one tile -> A1 (raw bytes).  Compact pools of TUs up to 32x32 stream in with cp.async (STREAM): the copy of tile k+1 is issued as soon as
   //      the stage-1 MMAs of tile k have consumed A1 and lands while the rest of tile k runs.
   constexpr bool PLANES = MODE == 1;
-  constexpr bool STREAMC = MODE == 0 && !S::ALIAS;
-  const bool STREAM = STREAMC && ( streamOn & 1 );
+  constexpr bool STREAM = MODE == 0 && !S::ALIAS;
   auto load_tile = [&]( int tile )
   {
 #pragma unroll
@@ -179,7 +178,7 @@ __global__ void __launch_bounds__( 128, N >= 32 ? 3 : 4 ) fwd_trquant_tc2_kernel
           *reinterpret_cast<uint4*>( sA1 + m * S::MT1 + c * S::LBO1 + tid * 16 ) = d;
         }
       }
-      else if( STREAMC && STREAM )
+      else if( STREAM )
       {
         const int16_t* src = resi + ( (size_t)( live ? tu : 0 ) * N + y ) * N;
         const uint32_t bytes = live ? 16u : 0u;                                  // 0: the 16 bytes are zero-filled
