@@ -394,6 +394,21 @@ int vvb_set_async( vvb_ctx* ctx, int enable ) { if( !ctx ) return VVB_ERR_ARG; c
 
 int vvb_launch_count( const vvb_ctx* ctx, uint64_t* k ) { if( !ctx || !k ) return VVB_ERR_ARG; *k = ctx->launches; return VVB_OK; }
 
+#ifdef VVB_PYR_PHASES
+// phase-timing build only (tools/pyr_phases.py): copies the pyramid kernel's per-level phase sums (3 levels x (PYR_NPHASE spans in ns, root count)) out after
+// the context's stream has finished, then clears them
+int vvb_pyr_phases_read( vvb_ctx* ctx, unsigned long long* out )
+{
+  if( !ctx || !out ) return VVB_ERR_ARG;
+  CU( cudaSetDevice( ctx->device ) );
+  CU( cudaStreamSynchronize( ctx->stream ) );
+  CU( cudaMemcpyFromSymbol( out, g_pyrPhaseNs, sizeof( g_pyrPhaseNs ) ) );
+  static const unsigned long long zero[3][PYR_NPHASE + 1] = {};
+  CU( cudaMemcpyToSymbol( g_pyrPhaseNs, zero, sizeof( zero ) ) );
+  return VVB_OK;
+}
+#endif
+
 // window staging of the dense search: 1 = TMA (cp.async.bulk.tensor.2d, default when available), 0 = load/store loop
 int vvb_set_tma_staging( vvb_ctx* ctx, int enable )
 {
@@ -870,7 +885,10 @@ static int pyramidV2LaunchLevel( vvb_ctx* ctx, int orgPlane, int refPlane, const
   }
   static const int forced = []{ const char* e = getenv( "VVB_PYR_THREADS" ); return e ? atoi( e ) : 0; }();     // tuning aid: fixed CTA size
   if( forced >= 64 && forced <= maxT && ( forced & 31 ) == 0 ) bd = forced;
-  sad_pyramid8_kernel<LV><<<nRoots, bd, (size_t) L.total, ctx->stream>>>( ctx->planes.p[orgPlane], ctx->planes.p[refPlane], lv, rootFirst, nx, ny, mp, L, 1u, 8u );
+  // 64x64 roots fill an SM each: one CTA per SM walks a run of consecutive roots and carries the shared half of each window to its right neighbour.
+  // Smaller roots share SMs and keep one CTA per root.
+  const int runs = LV == 4 ? std::min( nRoots, ctx->numSMs ) : nRoots;
+  sad_pyramid8_kernel<LV><<<runs, bd, (size_t) L.total, ctx->stream>>>( ctx->planes.p[orgPlane], ctx->planes.p[refPlane], lv, rootFirst, nRoots, nx, ny, mp, L, 1u, 8u );
   CHECK_LAUNCH( "sad_pyramid8_kernel" );
   return VVB_OK;
 }
