@@ -110,7 +110,8 @@ int vvb_fix_wsse_batch    ( vvb_ctx* ctx, const vvb_cand* cands, const uint32_t*
 int vvb_fix_wsse_batch_dev( vvb_ctx* ctx, const vvb_cand* dev_cands, const uint32_t* dev_weights, int n, uint64_t* dev_cost_out );
 
 /* ---- candidate-pool regime (RDO style): K candidate predictions per original block, each with its own
- * compact w x h buffer: pool[(b*K + k)*w*h ...].  One cost per (block, candidate); HBM streaming. ---------- */
+ * compact w x h buffer: pool[(b*K + k)*w*h ...].  One cost per (block, candidate); HBM streaming.  Costs above 32 bits
+ * (SSE of 128x64 blocks at 10 bits, of 32x32 at 12 bits) saturate at 0xffffffff; vvb_dist_batch returns them exactly. ---------- */
 typedef struct { int32_t x, y; } vvb_pos;
 int vvb_dist_pool    ( vvb_ctx* ctx, int dfunc, int org_plane, const vvb_pos* blocks, int n_blocks, int w, int h, int K,
                        const int16_t* pool, int sub_shift, uint32_t* cost_out /* n_blocks*K */ );
@@ -159,7 +160,8 @@ int vvb_sad_search_pyramid    ( vvb_ctx* ctx, int org_plane, int ref_plane, int 
                                 const int* counts, int base_w, const vvb_me_par* par, int nx, int ny, vvb_best* const* best_out /* [levels], host */ );
 
 /* Engine of vvb_sad_search_pyramid*: 1 (default) = one CTA per root block keeps every level on the SM (8x8 base blocks, no row sub-sampling, up to four
- * levels, window within shared memory; other cases use engine 0 automatically), 0 = one CTA per quad + cost-table sums through device memory.  Results are identical. */
+ * levels, planes of at most 10 bits, window within shared memory; other cases use engine 0 automatically), 0 = one CTA per quad + cost-table sums through
+ * device memory.  Results are identical. */
 int vvb_set_pyramid_engine( vvb_ctx* ctx, int engine );
 
 /* Fixed candidate set = the static point pattern of xTZ8PointDiamondSearch / raster scan
@@ -178,7 +180,8 @@ int vvb_sad_pattern_dev( vvb_ctx* ctx, int org_plane, int ref_plane, const vvb_b
 int vvb_set_tma_staging( vvb_ctx* ctx, int enable );
 
 /* Same candidate pattern with any distortion family (e.g. Hadamard integer refinement, InterSearch.cpp:2582,2630 and
- * xPatternRefinement :760-972, which add the MV rate the same way); cost_out holds the distortion only. */
+ * xPatternRefinement :760-972, which add the MV rate the same way); cost_out holds the distortion only.  A distortion above 32 bits (SSE of large
+ * blocks) is reported as 0xfffffffe in cost_out and best_out->sad; best_out->cost and the choice of the best point use the exact 64-bit value. */
 int vvb_cost_pattern    ( vvb_ctx* ctx, int dfunc, int org_plane, int ref_plane, const vvb_block* blocks, int n, int w, int h, const vvb_mv* pattern, int K,
                           const vvb_me_par* par, uint32_t* cost_out /* n*K, nullable */, vvb_best* best_out /* nullable */ );
 int vvb_cost_pattern_dev( vvb_ctx* ctx, int dfunc, int org_plane, int ref_plane, const vvb_block* dev_blocks, int n, int w, int h, const vvb_mv* dev_pattern, int K,

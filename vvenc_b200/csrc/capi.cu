@@ -845,12 +845,14 @@ static int sadSearchLaunch( vvb_ctx* ctx, int orgPlane, int refPlane, const vvb_
 #define LAUNCH_SS( T_, P_ ) LAUNCH_SS3( T_, P_, false )
 #define LAUNCH_SS3( T_, P_, K_ ) sad_search_kernel<T_, P_, K_><<<grid, bd, smem, ctx->stream>>>( ctx->planes.p[orgPlane], rp, dBlocks, n, w, h, nb == 2 ? 1 : 0, mp, tmap, ti, dTables, tableStride, dBest, \
                                                                                     pyr ? pyr->parents : nullptr, pyr ? pyr->best : nullptr, pyr ? pyr->tables : nullptr, pyr ? pyr->stride : 0 )
-  // 32-bit argmin keys in the pyramid base kernel when the largest possible parent cost (4 members' SAD + MV cost) leaves room for the raster order
+  // 32-bit argmin keys in the pyramid base kernel when the largest possible parent cost (4 members' SAD + MV cost) leaves room for the raster order.
+  // A pel difference is bounded by the wider of the two planes' bit depths.
   bool key32 = false;
   if( pyr )
   {
     int ob = 1; while( ( 1 << ob ) < maxNx * maxNy ) ob++;
-    const unsigned long long maxCost = 4ull * w * h * ( ( 1ull << rp.bitDepth ) - 1 ) + mp.tab.cost[VVB_MVCOST_ENTRIES - 1];
+    const int bd = std::max( ctx->planes.p[orgPlane].bitDepth, rp.bitDepth );
+    const unsigned long long maxCost = 4ull * w * h * ( ( 1ull << bd ) - 1 ) + mp.tab.cost[VVB_MVCOST_ENTRIES - 1];
     if( ob <= 16 && maxCost < ( 1ull << ( 32 - ob ) ) - 1 ) { key32 = true; mp.orderBits = ob; }
   }
   if( pyr && key32 ) { if( ti.enabled ) LAUNCH_SS3( true, true, true ); else LAUNCH_SS3( false, true, true ); }
@@ -893,12 +895,15 @@ static int pyramidV2LaunchLevel( vvb_ctx* ctx, int orgPlane, int refPlane, const
   return VVB_OK;
 }
 
-static bool pyramidV2Usable( const vvb_ctx* ctx, int refPlane, int levels, int baseW, const vvb_me_par* par, int nx, int ny, MePar& mp )
+// The kernel keeps the reference window's 8x8 box sums as uint16 lanes (64 * 1023 fits, 64 * 2047 does not): planes above 10 bits take engine 0.  The cost
+// bound takes the wider of the two bit depths, since a pel difference can reach either plane's maximum.
+static bool pyramidV2Usable( const vvb_ctx* ctx, int orgPlane, int refPlane, int levels, int baseW, const vvb_me_par* par, int nx, int ny, MePar& mp )
 {
   if( ctx->pyramidEngine != 1 || baseW != 8 || par->sub_shift != 0 || levels < 2 || levels > 4 ) return false;
+  const int bd = std::max( ctx->planes.p[orgPlane].bitDepth, ctx->planes.p[refPlane].bitDepth );
+  if( bd > 10 ) return false;
   int ob = 1; while( ( 1 << ob ) < nx * ny ) ob++;
-  const Plane& rp = ctx->planes.p[refPlane];
-  const unsigned long long maxCost16 = 4ull * 64 * ( ( 1ull << rp.bitDepth ) - 1 ) + mp.tab.cost[VVB_MVCOST_ENTRIES - 1];
+  const unsigned long long maxCost16 = 4ull * 64 * ( ( 1ull << bd ) - 1 ) + mp.tab.cost[VVB_MVCOST_ENTRIES - 1];
   if( ob > 16 || maxCost16 >= ( 1ull << ( 32 - ob ) ) || maxCost16 >= PYR_NEVER / 4 ) return false;
   const int total = levels == 4 ? pyr_smem<4>( nx, ny ).total : ( levels == 3 ? pyr_smem<3>( nx, ny ).total : pyr_smem<2>( nx, ny ).total );
   if( total > 227 * 1024 ) return false;
@@ -969,7 +974,7 @@ int vvb_sad_search_pyramid_dev( vvb_ctx* ctx, int orgPlane, int refPlane, int le
     MePar mp2;
     if( ( rc = makeMePar( ctx, par, mp2 ) ) ) return rc;
     if( ( rc = checkSearchShape( ctx, orgPlane, refPlane, baseW, baseW ) ) ) return rc;
-    if( pyramidV2Usable( ctx, refPlane, levels, baseW, par, nx, ny, mp2 ) )
+    if( pyramidV2Usable( ctx, orgPlane, refPlane, levels, baseW, par, nx, ny, mp2 ) )
     {
       PyrLevels lv; memset( &lv, 0, sizeof( lv ) );
       for( int l = 0; l < levels; l++ ) { lv.blocks[l] = dBlocks[l]; lv.best[l] = dBest[l]; }

@@ -310,6 +310,9 @@ __global__ void __launch_bounds__( 256 ) dist_list_kernel( const __grid_constant
   }
 }
 
+// uint32 cost outputs saturate: the SSE of a 128x64 block at 10 bits or of a 32x32 block at 12 bits exceeds 32 bits and must not wrap to a small cost
+__device__ __forceinline__ uint32_t sat_u32( unsigned long long v ) { return v < 0xffffffffull ? (uint32_t) v : 0xffffffffu; }
+
 // candidate pool: candidate (b,k) = compact w*h block at pool + (b*K+k)*w*h against org block b of a plane
 template<int G>
 __global__ void __launch_bounds__( 256 ) dist_pool_kernel( const __grid_constant__ Plane orgPlane, const vvb_pos* __restrict__ blocks, int nBlocks,
@@ -327,7 +330,7 @@ __global__ void __launch_bounds__( 256 ) dist_pool_kernel( const __grid_constant
     const int16_t* org = orgPlane.origin + (ptrdiff_t) p.y * orgPlane.stride + p.x;
     const int16_t* cur = pool + (size_t) i * area;
     const unsigned long long v = group_dist<G>( fam, org, orgPlane.stride, cur, w, w, h, subShift, lg );   // shuffles use the group's own lane mask
-    if( lg == 0 ) out[i] = (uint32_t) v;
+    if( lg == 0 ) out[i] = sat_u32( v );
   }
 }
 
@@ -415,7 +418,7 @@ __global__ void __launch_bounds__( 256, 3 ) sad_pool_stream_kernel( const __grid
         {
 #pragma unroll
           for( int m = G >> 1; m > 0; m >>= 1 ) acc64 += __shfl_xor_sync( mk, acc64, m );
-          if( lg == 0 ) out[(size_t) b * K + k] = (uint32_t) acc64;
+          if( lg == 0 ) out[(size_t) b * K + k] = sat_u32( acc64 );
         }
       }
     }
@@ -451,7 +454,7 @@ __global__ void __launch_bounds__( 256, 3 ) sad_pool_stream_kernel( const __grid
         {
 #pragma unroll
           for( int m = G >> 1; m > 0; m >>= 1 ) acc64 += __shfl_xor_sync( mk, acc64, m );
-          if( lg == 0 ) out[(size_t) b * K + k] = (uint32_t) acc64;
+          if( lg == 0 ) out[(size_t) b * K + k] = sat_u32( acc64 );
         }
       }
     }

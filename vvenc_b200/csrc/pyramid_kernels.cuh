@@ -345,7 +345,8 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
       }
     }
     __syncthreads();
-    // ---- box sums V[r][c] = sum_{y<8} Hs[r+y][c]  (uint16: 64 * 1023 fits); a thread slides down a chunk of rows of one column pair
+    // ---- box sums V[r][c] = sum_{y<8} Hs[r+y][c]  (uint16: 64 * 1023 fits; pyramidV2Usable sends planes above 10 bits to engine 0); a thread slides down
+    // a chunk of rows of one column pair
     {
       const int cPairs = L.vPitch >> 1, chunk = 16, nChunks = ( L.vRows + chunk - 1 ) / chunk;
       const uint32_t* Hs32 = reinterpret_cast<const uint32_t*>( Hs );

@@ -633,9 +633,11 @@ __global__ void __launch_bounds__( 128 ) cost_pattern_kernel( const __grid_const
     uint32_t sad = 0xffffffffu;
     if( inside )        // uniform per group
     {
+      // the decision uses the full 64-bit distortion (an SSE may exceed 32 bits); the uint32 outputs saturate below the "outside" marker
       const int16_t* cur = refPlane.origin + (ptrdiff_t)( blk.y + my ) * refPlane.stride + blk.x + mx;
-      sad = (uint32_t) group_dist<G>( fam, org, orgPlane.stride, cur, refPlane.stride, w, h, par.subShift, lg );
-      const unsigned long long c = (unsigned long long) sad + mv_cost( par, sMv, mx, my, blk.pred_hor, blk.pred_ver );
+      const unsigned long long dist = group_dist<G>( fam, org, orgPlane.stride, cur, refPlane.stride, w, h, par.subShift, lg );
+      sad = dist < 0xfffffffeull ? (uint32_t) dist : 0xfffffffeu;
+      const unsigned long long c = dist + mv_cost( par, sMv, mx, my, blk.pred_hor, blk.pred_ver );
       if( better( c, (uint32_t) k, bestCost, bestOrder ) ) { bestCost = c; bestOrder = (uint32_t) k; bestSad = sad; }
     }
     if( sadOut && lg == 0 ) sadOut[(size_t) blockIdx.x * K + k] = sad;
