@@ -366,7 +366,11 @@ int vvb_tu_roundtrip_dev( vvb_ctx* ctx, const vvb_tu_par* par, const int16_t* de
 int vvb_tu_roundtrip_planes_dev( vvb_ctx* ctx, const vvb_tu_par* par, int org_plane, int pred_plane, const vvb_block* dev_blocks, int n,
                           int16_t* dev_q, int16_t* dev_reco, vvb_tu_result* dev_res, uint8_t* dev_need_rdoq );
 
-/* ---- MCTF block matching (CommonLib/MCTF.cpp:122-257 via MCTF::motionErrorLuma :1099-1164) ----------------- */
+/* ---- MCTF block matching (CommonLib/MCTF.cpp:122-257 via MCTF::motionErrorLuma :1099-1164) -----------------
+ * Every MCTF entry (error batch, search grid, calc_var, estimate_level, estimate_pyramid, apply) takes planes of up to 10 bits and returns
+ * VVB_ERR_UNSUPPORTED when the original or the reference is wider (MCTF.cpp:1313 CHECKD).  Errors are exact SSEs while they fit int32 and saturate to
+ * 0x7fffffff above it (a 64x64 block at 10 bits reaches 4096 * 1023^2): the reference stops summing as soon as its sum passes the best error, so a
+ * saturated candidate never beats a finite best under the strict `error < best.error` chains, which is the reference's decision. */
 typedef struct { int32_t x, y; int32_t mvx, mvy; /* 1/16 pel */ uint16_t w, h; } vvb_mctf_cand;   /* 20 bytes */
 int vvb_mctf_error_batch    ( vvb_ctx* ctx, int org_plane, int ref_plane, const vvb_mctf_cand* cands, int n, int low_res_filter /* 4-tap */, int32_t* err_out );
 int vvb_mctf_error_batch_dev( vvb_ctx* ctx, int org_plane, int ref_plane, const vvb_mctf_cand* dev_cands, int n, int low_res_filter, int32_t* dev_err_out );

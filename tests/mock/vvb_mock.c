@@ -108,6 +108,7 @@ int vvb_mctf_error_batch( vvb_ctx* c, int orgPlane, int refPlane, const vvb_mctf
   if( !c ) return VVB_ERR_ARG;
   mock_plane* o = plane( c, orgPlane ); mock_plane* r = plane( c, refPlane );
   if( !o || !r || !cands || !errOut || n < 0 ) return fail( c, VVB_ERR_ARG, "bad mctf arguments" );
+  if( o->bitDepth > 10 || r->bitDepth > 10 ) return fail( c, VVB_ERR_UNSUPPORTED, "MCTF supports up to 10 bit (MCTF.cpp:1313 CHECKD)" );
   for( int i = 0; i < n; i++ )
     if( cands[i].w < 8 || cands[i].h < 8 || cands[i].w > 64 || cands[i].h > 64 || ( cands[i].w & 7 ) || ( cands[i].h & 7 ) ) return fail( c, VVB_ERR_UNSUPPORTED, "MCTF blocks are multiples of 8 up to 64" );
   for( int i = 0; i < n; i++ )
@@ -124,6 +125,7 @@ int vvb_mctf_search_grid( vvb_ctx* c, int orgPlane, int refPlane, const vvb_mctf
   if( !c ) return VVB_ERR_ARG;
   mock_plane* o = plane( c, orgPlane ); mock_plane* r = plane( c, refPlane );
   if( !o || !r || !blocks || !errOut || n < 0 ) return fail( c, VVB_ERR_ARG, "bad mctf grid arguments" );
+  if( o->bitDepth > 10 || r->bitDepth > 10 ) return fail( c, VVB_ERR_UNSUPPORTED, "MCTF supports up to 10 bit (MCTF.cpp:1313 CHECKD)" );
   if( step < 1 || step > 16 || radius < 0 || radius > 8 ) return fail( c, VVB_ERR_ARG, "MCTF grid: step 1..16 (1/16 pel), radius 0..8 steps" );
   for( int i = 0; i < n; i++ )
     if( blocks[i].w < 8 || blocks[i].h < 8 || blocks[i].w > 64 || blocks[i].h > 64 || ( blocks[i].w & 7 ) || ( blocks[i].h & 7 ) ) return fail( c, VVB_ERR_UNSUPPORTED, "MCTF blocks are multiples of 8 up to 64" );
@@ -210,6 +212,7 @@ int vvb_mctf_calc_var( vvb_ctx* c, int planeId, const vvb_mctf_cand* blocks, int
   if( !c ) return VVB_ERR_ARG;
   mock_plane* o = plane( c, planeId );
   if( !o || !blocks || !varOut || n < 0 ) return fail( c, VVB_ERR_ARG, "bad calc_var arguments" );
+  if( o->bitDepth > 10 ) return fail( c, VVB_ERR_UNSUPPORTED, "MCTF supports up to 10 bit (MCTF.cpp:1313 CHECKD)" );
   for( int i = 0; i < n; i++ ) varOut[i] = orc_mctf_calc_var( o->origin + (ptrdiff_t) blocks[i].y * o->stride + blocks[i].x, o->stride, blocks[i].w, blocks[i].h );
   c->calls++;
   return VVB_OK;

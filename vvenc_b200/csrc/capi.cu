@@ -1809,6 +1809,13 @@ static int mctfLaunch( vvb_ctx* ctx, const Plane& po, const Plane& pr, const vvb
   return VVB_OK;
 }
 
+// the MCTF filters and errors are defined up to 10 bits (MCTF.cpp:1313 CHECKD; 64 x 64 SSEs above it leave 32 bits): the wider of the two planes decides
+static int mctfBitDepthOk( vvb_ctx* ctx, int orgPlane, int refPlane )
+{
+  if( std::max( ctx->planes.p[orgPlane].bitDepth, ctx->planes.p[refPlane].bitDepth ) > 10 ) return fail( ctx, VVB_ERR_UNSUPPORTED, "MCTF supports up to 10 bit (MCTF.cpp:1313 CHECKD)" );
+  return VVB_OK;
+}
+
 int vvb_mctf_hint( vvb_ctx* ctx, int maxBlockDim )
 {
   if( !ctx || maxBlockDim < 8 || maxBlockDim > 64 ) return fail( ctx, VVB_ERR_ARG, "MCTF block dimension hint must be 8..64" );
@@ -1820,6 +1827,7 @@ int vvb_mctf_error_batch_dev( vvb_ctx* ctx, int orgPlane, int refPlane, const vv
 {
   if( !ctx || !dCands || !dErr || n < 0 ) return fail( ctx, VVB_ERR_ARG, "bad arguments" );
   if( !validPlane( ctx, orgPlane ) || !validPlane( ctx, refPlane ) ) return fail( ctx, VVB_ERR_ARG, "unknown plane" );
+  if( int rc = mctfBitDepthOk( ctx, orgPlane, refPlane ) ) return rc;
   if( n == 0 ) return VVB_OK;
   return mctfLaunch( ctx, ctx->planes.p[orgPlane], ctx->planes.p[refPlane], dCands, n, lowRes, ctx->mctfMaxDim, dErr );
 }
@@ -1832,6 +1840,7 @@ int vvb_mctf_error_batch( vvb_ctx* ctx, int orgPlane, int refPlane, const vvb_mc
       return fail( ctx, VVB_ERR_UNSUPPORTED, "MCTF blocks are multiples of 8 up to 64 (MCTF.cpp:1113-1118)" );
   if( n == 0 ) return VVB_OK;
   if( !validPlane( ctx, orgPlane ) || !validPlane( ctx, refPlane ) ) return fail( ctx, VVB_ERR_ARG, "unknown plane" );
+  if( int rc = mctfBitDepthOk( ctx, orgPlane, refPlane ) ) return rc;
   int maxDim = 8;
   for( int i = 0; i < n; i++ ) maxDim = std::max( maxDim, (int) std::max( cands[i].w, cands[i].h ) );
   const vvb_mctf_cand* dC; int32_t* dE;
@@ -1954,6 +1963,7 @@ int vvb_mctf_calc_var_dev( vvb_ctx* ctx, int plane, const vvb_mctf_cand* dBlocks
 {
   if( !ctx || !dBlocks || !dVar || n < 0 ) return fail( ctx, VVB_ERR_ARG, "bad arguments" );
   if( !validPlane( ctx, plane ) ) return fail( ctx, VVB_ERR_ARG, "unknown plane" );
+  if( int rc = mctfBitDepthOk( ctx, plane, plane ) ) return rc;
   if( n == 0 ) return VVB_OK;
   CU( cudaSetDevice( ctx->device ) );
   mctf_calc_var_kernel<<<( n + 3 ) / 4, 128, 0, ctx->stream>>>( ctx->planes.p[plane], dBlocks, n, dVar );
@@ -1987,7 +1997,7 @@ static int mctfGridArgs( vvb_ctx* ctx, int orgPlane, int refPlane, int n, int st
 {
   if( n < 0 || step < 1 || step > 16 || radius < 0 || radius > 8 ) return fail( ctx, VVB_ERR_ARG, "MCTF grid: step 1..16 (1/16 pel), radius 0..8 steps" );
   if( !validPlane( ctx, orgPlane ) || !validPlane( ctx, refPlane ) ) return fail( ctx, VVB_ERR_ARG, "unknown plane" );
-  return VVB_OK;
+  return mctfBitDepthOk( ctx, orgPlane, refPlane );
 }
 
 int vvb_mctf_search_grid_dev( vvb_ctx* ctx, int orgPlane, int refPlane, const vvb_mctf_cand* dBlocks, int n, int step, int radius, int lowRes, int32_t* dErr )
@@ -2098,7 +2108,7 @@ int mctfLevel( vvb_ctx* ctx, const Plane& po, const Plane& pr, int width, int he
   }
   {
     const int maxDim = std::max( 8, std::min( 64, ( bs + 7 ) & ~7 ) );
-    const MctfSmem L = mctf_smem( maxDim );
+    const MctfSmem L = mctf_wave_smem( maxDim );
     mctf_wave_kernel<<<g.byn, MCTF_WAVE_WARPS * 32, (size_t) MCTF_WAVE_WARPS * L.warpWords * 4, ctx->stream>>>( po, pr, g, lowRes ? 1 : 0, maxDim, a.best, a.progress );
     CHECK_LAUNCH( "mctf_wave_kernel" );
   }
@@ -2121,6 +2131,7 @@ int vvb_mctf_estimate_level_dev( vvb_ctx* ctx, int orgPlane, int refPlane, const
   if( !validPlane( ctx, orgPlane ) || !validPlane( ctx, refPlane ) ) return fail( ctx, VVB_ERR_ARG, "unknown plane" );
   if( ( lp->block_size != 8 && lp->block_size != 16 && lp->block_size != 32 && lp->block_size != 64 ) || lp->search_pattern < 0 || lp->search_pattern > 2 || lp->out_w < 1 || lp->out_h < 1 )
     return fail( ctx, VVB_ERR_ARG, "bad level parameters" );
+  if( int rc = mctfBitDepthOk( ctx, orgPlane, refPlane ) ) return rc;
   const Plane& po = ctx->planes.p[orgPlane];
   CU( cudaSetDevice( ctx->device ) );
   const int bxn = ( po.width - 8 ) / lp->block_size + 1, byn = ( po.height - 8 ) / lp->block_size + 1;
@@ -2146,6 +2157,7 @@ int vvb_mctf_estimate_pyramid_dev( vvb_ctx* ctx, int orgPlane, int refPlane, con
   if( !ctx || !pp || !dOut ) return fail( ctx, VVB_ERR_ARG, "bad arguments" );
   if( !validPlane( ctx, orgPlane ) || !validPlane( ctx, refPlane ) ) return fail( ctx, VVB_ERR_ARG, "unknown plane" );
   if( ( pp->unit_size != 8 && pp->unit_size != 16 && pp->unit_size != 32 ) || pp->search_pattern < 0 || pp->search_pattern > 2 ) return fail( ctx, VVB_ERR_ARG, "bad pyramid parameters" );
+  if( int rc = mctfBitDepthOk( ctx, orgPlane, refPlane ) ) return rc;
   CU( cudaSetDevice( ctx->device ) );
   const Plane po0 = ctx->planes.p[orgPlane], pr0 = ctx->planes.p[refPlane];
   const int W = po0.width, H = po0.height, u = pp->unit_size, nSub = pp->add_level ? 3 : 2, margin = 128;

@@ -25,22 +25,28 @@ __device__ __constant__ short c_mctfF4[16][4] = {
 // memory, both filter passes run on IDP.2A.  Pel pairs are packed along x for the horizontal pass and along y (row pairs) for the
 // vertical pass; a 6-tap output whose first pel sits in the low half of a word takes 3 IDP.2A ("E"), one that starts in the high half
 // takes 4 with zero-padded taps ("O").  The 4-tap filters are embedded as (0, t0, t1, t2, t3, 0): same pels, same sums.
-// Taps fit int8 (|t| <= 64), pels and clipped intermediates fit int16, sums are int32 exactly as MCTF.cpp:147-257.
+// Taps fit int8 (|t| <= 64), pels and clipped intermediates fit int16.  A lane's partial sum covers at most 128 pels and fits int32; the warp sum is
+// reduced unsigned, which is exact up to 64 x 64 pels at 10 bits (4096 * 1023^2 < 2^32), and the kernels saturate it to 0x7fffffff where they store int32.
+// The reference's sums are int32 too, but its early exit (MCTF.cpp:138, 196, 250) returns before they can wrap; a saturated error loses every strict
+// `error < best.error` against a finite best, as the reference's partial sum does.
 struct MctfSmem { int regionPitch, regionWords, t2Words, warpWords; };
-__host__ __device__ inline MctfSmem mctf_smem( int maxDim )
+__host__ __device__ inline MctfSmem mctf_smem( int maxW, int maxH )
 {
   MctfSmem m;
-  m.regionPitch = maxDim / 2 + 4;                                // words per region row: w + 5 pels + alignment, rounded up
-  m.regionWords = ( maxDim + 6 ) * m.regionPitch;                // h + 5 rows, + 1 so that the last row pair is addressable
-  m.t2Words     = ( ( maxDim + 6 ) / 2 ) * maxDim;               // row pairs x w
+  m.regionPitch = maxW / 2 + 4;                                  // words per region row: w + 5 pels + alignment, rounded up
+  m.regionWords = ( maxH + 6 ) * m.regionPitch;                  // h + 5 rows, + 1 so that the last row pair is addressable
+  m.t2Words     = ( ( maxH + 6 ) / 2 ) * maxW;                   // row pairs x w
   m.warpWords   = m.regionWords + m.t2Words;
   return m;
 }
+__host__ __device__ inline MctfSmem mctf_smem( int maxDim ) { return mctf_smem( maxDim, maxDim ); }
+
+__device__ __forceinline__ int32_t mctf_sat32( unsigned long long e ) { return (int32_t)( e < 0x7fffffffull ? e : 0x7fffffffull ); }
 
 __device__ __forceinline__ int mctf_div( int i, float inv ) { return __float2int_rz( ( (float) i + 0.5f ) * inv ); }   // exact for i < 2^20, divisors <= 64
 
-// motionErrorLuma of one candidate by one warp (no early exit); region / t2: the warp's slices of shared memory (mctf_smem); every lane returns the error
-__device__ __forceinline__ int mctf_warp_error( const Plane& orgPlane, const Plane& refPlane, const vvb_mctf_cand& c, int tap4, const MctfSmem& L, uint32_t* region, uint32_t* t2, int lane )
+// motionErrorLuma of one candidate by one warp (no early exit, unsaturated); region / t2: the warp's slices of shared memory (mctf_smem); every lane returns the error
+__device__ __forceinline__ unsigned mctf_warp_error( const Plane& orgPlane, const Plane& refPlane, const vvb_mctf_cand& c, int tap4, const MctfSmem& L, uint32_t* region, uint32_t* t2, int lane )
 {
   const int PW = L.regionPitch;
   const int maxv = ( 1 << refPlane.bitDepth ) - 1;
@@ -129,9 +135,7 @@ __device__ __forceinline__ int mctf_warp_error( const Plane& orgPlane, const Pla
 #undef VVB_O
 #undef VVB_RC
   }
-#pragma unroll
-  for( int m = 16; m > 0; m >>= 1 ) err += __shfl_xor_sync( 0xffffffffu, err, m );
-  return err;
+  return __reduce_add_sync( 0xffffffffu, (unsigned) err );
 }
 
 __global__ void __launch_bounds__( MCTF_WARPS * 32 ) mctf_error_packed_kernel( const __grid_constant__ Plane orgPlane, const __grid_constant__ Plane refPlane,
@@ -147,8 +151,8 @@ __global__ void __launch_bounds__( MCTF_WARPS * 32 ) mctf_error_packed_kernel( c
   {
     const vvb_mctf_cand c = cands[ci];
     if( c.w > maxDim || c.h > maxDim || ( ( c.w | c.h ) & 1 ) ) { if( lane == 0 ) out[ci] = -1; continue; }     // outside the promised geometry
-    const int err = mctf_warp_error( orgPlane, refPlane, c, tap4, L, region, t2, lane );
-    if( lane == 0 ) out[ci] = err;
+    const unsigned err = mctf_warp_error( orgPlane, refPlane, c, tap4, L, region, t2, lane );
+    if( lane == 0 ) out[ci] = mctf_sat32( err );
   }
 }
 
@@ -188,7 +192,7 @@ __global__ void __launch_bounds__( 256 ) mctf_grid_kernel( const __grid_constant
   uint32_t* win  = sGrid;
   uint32_t* hbuf = win + L.winWords;
   uint32_t* orgP = hbuf + L.hWords;
-  int*      sErr = reinterpret_cast<int*>( orgP + L.orgWords );
+  unsigned* sErr = orgP + L.orgWords;                                       // exact up to 64 x 64 pels at 10 bits (4096 * 1023^2 < 2^32)
   int4*     sTap = reinterpret_cast<int4*>( sGrid + L.tapOff );           // [2 * K1]: x columns, then y rows
   const int tid = threadIdx.x, T = blockDim.x;
   const int K1 = 2 * radius + 1, K = K1 * K1;
@@ -284,7 +288,7 @@ __global__ void __launch_bounds__( 256 ) mctf_grid_kernel( const __grid_constant
           {
             const int q = ( ( blk.mvy + ( j - radius ) * step ) >> 4 ) - dyMin + 2 * yp;
             const int4 ty = sTap[K1 + j];
-            int err = 0;
+            unsigned err = 0;
             if( act )
             {
               const uint32_t* tp = hx + ( q >> 1 ) * w;
@@ -310,7 +314,7 @@ __global__ void __launch_bounds__( 256 ) mctf_grid_kernel( const __grid_constant
           const int q0 = ( mvy >> 4 ) - dyMin;                                 // first filtered row of output row 0
           const int4 ty = sTap[K1 + j];
           const int yFA = ty.x, yFB = ty.y, yGA = ty.z, yGB = ty.w;
-          int err = 0;
+          unsigned err = 0;
           for( int p = tid; p < hh * w; p += T )
           {
             const int yp = mctf_div( p, invW ), x = p - yp * w;
@@ -336,7 +340,7 @@ __global__ void __launch_bounds__( 256 ) mctf_grid_kernel( const __grid_constant
 #undef VVB_RC
 #undef VVB_TAPS
     __syncthreads();
-    for( int k = tid; k < K; k += T ) out[(size_t) b * K + k] = sErr[k];
+    for( int k = tid; k < K; k += T ) out[(size_t) b * K + k] = mctf_sat32( sErr[k] );
   }
 }
 

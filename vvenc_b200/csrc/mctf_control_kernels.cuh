@@ -111,14 +111,17 @@ __global__ void mctf_select_grid_kernel( MctfGeom g, const int32_t* __restrict__
 // candidates of a block -- the final vector of the block above, then that of the block to the left -- are evaluated side by side: four warps each, a warp
 // takes a horizontal quarter of the block (the error is a sum over pels, and a pel's interpolation only reads its own neighbourhood, so the quarters add up to
 // motionErrorLuma of the block exactly).  A candidate whose vector equals the block's current vector (or the other candidate's) cannot win the strict
-// `error < best.error` and is not evaluated -- on smooth fields that is most of them.
+// `error < best.error` and is not evaluated -- on smooth fields that is most of them.  The four quarters add up in 64 bits and saturate to 0x7fffffff.
 #define MCTF_WAVE_WARPS 8
+// a warp's slice holds one quarter: up to maxDim x maxDim / 4 pels (8 warps of 64 x 64 regions would not fit the 100 KB the kernel is given)
+__host__ __device__ inline MctfSmem mctf_wave_smem( int maxDim ) { return mctf_smem( maxDim, maxDim >> 2 ); }
 __global__ void __launch_bounds__( MCTF_WAVE_WARPS * 32 ) mctf_wave_kernel( const __grid_constant__ Plane orgPlane, const __grid_constant__ Plane refPlane, MctfGeom g, int tap4, int maxDim,
                                                                             MctfBest* best, int* progress )
 {
   extern __shared__ __align__( 16 ) uint32_t sWave[];
-  __shared__ int sRow, sErr[MCTF_WAVE_WARPS];
-  const MctfSmem L = mctf_smem( maxDim );
+  __shared__ int sRow;
+  __shared__ unsigned sErr[MCTF_WAVE_WARPS];
+  const MctfSmem L = mctf_wave_smem( maxDim );
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   uint32_t* region = sWave + warp * L.warpWords; uint32_t* t2 = region + L.regionWords;
   if( threadIdx.x == 0 ) sRow = atomicAdd( &progress[0], 1 );
@@ -149,12 +152,12 @@ __global__ void __launch_bounds__( MCTF_WAVE_WARPS * 32 ) mctf_wave_kernel( cons
       const int q = warp & 3, sh = H >> 2;                // H is a multiple of 8: quarters of an even number of rows
       vvb_mctf_cand c; c.x = X; c.y = Y + q * sh; c.w = (uint16_t) W; c.h = (uint16_t) sh;
       c.mvx = warp < 4 ? up.x : left.x; c.mvy = warp < 4 ? up.y : left.y;
-      const int e = mctf_warp_error( orgPlane, refPlane, c, tap4, L, region, t2, lane );
+      const unsigned e = mctf_warp_error( orgPlane, refPlane, c, tap4, L, region, t2, lane );
       if( lane == 0 ) sErr[warp] = e;
     }
     __syncthreads();
-    if( needUp )   { const int e = sErr[0] + sErr[1] + sErr[2] + sErr[3]; if( e < b.e ) { b.e = e; b.x = up.x; b.y = up.y; } }
-    if( needLeft ) { const int e = sErr[4] + sErr[5] + sErr[6] + sErr[7]; if( e < b.e ) { b.e = e; b.x = left.x; b.y = left.y; } }
+    if( needUp )   { const int e = mctf_sat32( (unsigned long long) sErr[0] + sErr[1] + sErr[2] + sErr[3] ); if( e < b.e ) { b.e = e; b.x = up.x; b.y = up.y; } }
+    if( needLeft ) { const int e = mctf_sat32( (unsigned long long) sErr[4] + sErr[5] + sErr[6] + sErr[7] ); if( e < b.e ) { b.e = e; b.x = left.x; b.y = left.y; } }
     left = b;
     if( threadIdx.x == 0 )
     {
@@ -173,7 +176,7 @@ __global__ void __launch_bounds__( MCTF_WAVE_WARPS * 32 ) mctf_wave_kernel( cons
 //             ( dp2a.lo against the low bytes, dp2a.hi against the high bytes );
 //   sum r^2   box sums of the squared window by two sliding passes, shared by all candidates;
 //   sum o^2   once per block.
-// Same table layout as mctf_grid_kernel (out[b][j][i], displacement centre + (i - r, j - r) * 16).
+// Same table layout as mctf_grid_kernel (out[b][j][i], displacement centre + (i - r, j - r) * 16); the exact 64-bit SSE saturates to 0x7fffffff.
 struct MctfIntSmem { int orgWords, pitch, rows, planeWords, sqPitch, total; };
 __host__ __device__ inline MctfIntSmem mctf_int_smem( int maxDim, int radius )
 {
@@ -275,7 +278,7 @@ __global__ void __launch_bounds__( 128 ) mctf_int_grid_kernel( const __grid_cons
         }
       unsigned long long cross = (unsigned long long) lo + 256ull * hi;
       for( int m = 16; m > 0; m >>= 1 ) cross += __shfl_xor_sync( 0xffffffffu, cross, m );
-      if( lane == 0 ) out[(size_t) b * K1 * K1 + c] = (int32_t)(long long)( ooAll + (unsigned long long) sV[j * L.sqPitch + i0] - 2ull * cross );
+      if( lane == 0 ) out[(size_t) b * K1 * K1 + c] = mctf_sat32( ooAll + (unsigned long long) sV[j * L.sqPitch + i0] - 2ull * cross );
     }
   }
 }
