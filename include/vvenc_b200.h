@@ -197,12 +197,18 @@ int vvb_blocks_set_start_dev( vvb_ctx* ctx, vvb_block* dev_blocks, const vvb_bes
  * (TrQuant::xInvLfnst, TrQuant.cpp:838-940: the first 16 scan positions through the transposed kernel, then xIT over the top-left 8x8 / 4x4, :590-602); the levels
  * are expected as a bitstream carries them, zero beyond scan position 7 (4x4, 8x8) or 15.
  * deltaU (Quant.cpp:221), whose only consumer is the sign-bit hiding of the same call, stays on the device: with sign_hiding set the returned levels are the
- * ones Quant::quant leaves after xSignBitHidingHDQ (abs_sum stays QuantCore's sum, as uiAbsSum does; last_pos follows the hiding step). */
+ * ones Quant::quant leaves after xSignBitHidingHDQ (abs_sum stays QuantCore's sum, as uiAbsSum does; last_pos follows the hiding step).
+ * Levels are clipped to -32768..32767; abs_sum is QuantCore's int32 sum of the unclipped magnitudes, so it may exceed the sum of the returned levels.
+ * The results equal the reference for residuals within +-(2^bit_depth - 1) (org - pred of in-range pels) at any QP, where abs_sum stays below 2^24.  Beyond that
+ * range (int16 residuals above the bit depth) the reference's own int32 transform sums can overflow (64 x 64 at 8 bits: 64 * 90 * 2^22 > 2^31 in the second
+ * stage), so it has no defined result there.  The dequantiser of dependent quantisation (vvb_inv_trquant with dep_quant) forms qIdx = 2 * level -+ (state >> 1) in 32 bits
+ * and the coefficient in 64 bits before the 16-bit clip, as DepQuant.cpp:616-618 does, so levels at the int16 extremes dequantise exactly. */
 typedef struct
 {
   int32_t w, h;                /* TU size, each in {4,8,16,32,64}                               */
   int32_t tr_hor, tr_ver;      /* 0 DCT-II, 1 DCT-VIII, 2 DST-VII (enum TransType)                */
-  int32_t bit_depth;           /* 8 or 10                                                         */
+  int32_t bit_depth;           /* 8..12 for vvb_fwd_trquant*, vvb_inv_trquant*, vvb_tu_roundtrip* and vvb_search_refine_tu; 8 or 10 for vvb_dep_quant and the
+                                  vvb_rdoq* entries.  Anything else: VVB_ERR_UNSUPPORTED                                                                            */
   int32_t qp;                  /* CU QP (cu.qp); +6*(bit_depth-8) applied inside (Quant.cpp:99)   */
   int32_t is_irap;             /* slice->isIRAP(): rounding offset 171 vs 85 (Quant.cpp:772)      */
   int32_t dep_quant;           /* slice->depQuantEnabled: the QP of need_rdoq (Quant.cpp:852-855); vvb_inv_trquant then dequantises as DepQuant::dequant does
