@@ -233,7 +233,9 @@ int vvb_fwd_trquant_dev( vvb_ctx* ctx, const vvb_tu_par* par, const int16_t* dev
 /* Transform engine of vvb_fwd_trquant*, vvb_inv_trquant* and vvb_tu_roundtrip*: 0 = CUDA-core IDP.2A kernels for every shape; any other value (default) = the
  * raw-byte wgmma engines (the MMAs read the bytes of the int16 residual / int32 stage-1 values as u8 / s8 against zero-interleaved matrices, quantiser in
  * registers) where they apply: square 8..64 TUs without LFNST or transform skip (forward: also without sign-bit hiding); CUDA cores elsewhere.
- * Both settings are bit-exact. */
+ * The raw-byte engines move TU data in 16-byte units, so a _dev call takes them only when every TU buffer it is given (residual, original and prediction
+ * pools, levels, coefficients, residual and reconstruction outputs; null ones aside) is 16-byte aligned.  Buffers that are only 8-byte aligned run on the
+ * CUDA-core kernels, which need no more than that.  Both settings are bit-exact. */
 int vvb_set_tensor_transform( vvb_ctx* ctx, int enable );
 /* Residual formed on the device: resi = org(x,y) - pred(x+start_x, y+start_y) for each TU position (PelBuf::subtract, IntraSearch.cpp:1328) */
 int vvb_fwd_trquant_planes    ( vvb_ctx* ctx, const vvb_tu_par* par, int org_plane, int pred_plane, const vvb_block* blocks, int n,

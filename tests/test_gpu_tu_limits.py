@@ -611,6 +611,98 @@ def test_search_refine_tu_at_12_bits(eng):
     assert clipped > 0
 
 
+# ---------------------------------------------------------------------------------------------------- _dev buffers 8- but not 16-byte aligned
+DEV_ENTRIES = ('fwd', 'fwd_planes', 'inv', 'rt')
+
+
+def dev_case(eng, w, entry, off):
+    """(call, expected) of one _dev entry on square w x w TUs at 10 bits and the lowest QP, with every pool and output `off` bytes into its own torch allocation
+    (the block list stays at the start of its own).  call() returns the outputs as numpy arrays; the plane form reads org / pred from planes 30 / 31."""
+    import torch
+    import vvenc_b200 as V
+    import vvenc_b200._lib as L
+    bd = 10; qp = qp_ends(bd)[0]
+    par = eng.tu_par(w, w, 0, 0, bd, qp, True, False)
+    resi = worst_residuals(w, w, 0, 0, bd, w)
+    n = len(resi)
+    keep, outs = [], {}
+
+    def dev_in(a):
+        raw = torch.from_numpy(np.frombuffer(np.ascontiguousarray(a).tobytes(), np.uint8).copy())
+        t = torch.zeros(raw.numel() + 16, dtype=torch.uint8, device='cuda')
+        t[off:off + raw.numel()] = raw.cuda()
+        keep.append(t)
+        return ctypes.c_void_p(t.data_ptr() + off)
+
+    def dev_out(name, dt, shape):
+        nb = int(np.prod(shape)) * np.dtype(dt).itemsize
+        t = torch.zeros(nb + 16, dtype=torch.uint8, device='cuda')
+        outs[name] = (t, dt, shape, nb)
+        return ctypes.c_void_p(t.data_ptr() + off)
+
+    def fwd_outs():
+        return (dev_out('coef', np.int32, (n, w, w)), dev_out('q', np.int16, (n, w, w)), dev_out('abs_sum', np.int32, (n,)), dev_out('last_pos', np.int32, (n,)),
+                dev_out('need_rdoq', np.uint8, (n,)))
+
+    lib, h, pp = eng.lib, eng.h, ctypes.byref(par)
+    if entry == 'fwd':
+        args = (pp, dev_in(resi), n) + fwd_outs()
+        fn, exp = lib.vvb_fwd_trquant_dev, fwd_oracle(w, w, 0, 0, bd, qp, 1, 0, resi)
+    elif entry == 'fwd_planes':
+        W, H, m = 192, 128, 16
+        org, pred = _planes(bd, W, H, m, w)
+        eng.upload_plane(30, org, W, H, m, bd); eng.upload_plane(31, pred, W, H, m, bd)
+        rs = np.random.RandomState(w)
+        B = np.zeros(n, dtype=V.BLOCK_DT)
+        B['x'] = rs.randint(0, W - w + 1, n); B['y'] = rs.randint(0, H - w + 1, n); B['start_x'] = rs.randint(-m, m + 1, n); B['start_y'] = rs.randint(-m, m + 1, n)
+        o = np.stack([org[m + b['y']:m + b['y'] + w, m + b['x']:m + b['x'] + w] for b in B])
+        p = np.stack([pred[m + b['y'] + b['start_y']:m + b['y'] + b['start_y'] + w, m + b['x'] + b['start_x']:m + b['x'] + b['start_x'] + w] for b in B])
+        d_blk = torch.from_numpy(np.frombuffer(B.tobytes(), np.uint8).copy()).cuda()
+        keep.append(d_blk)
+        args = (pp, 30, 31, ctypes.c_void_p(d_blk.data_ptr()), n) + fwd_outs()
+        fn, exp = lib.vvb_fwd_trquant_planes_dev, fwd_oracle(w, w, 0, 0, bd, qp, 1, 0, (o.astype(np.int32) - p).astype(np.int16))
+    elif entry == 'inv':
+        q = extreme_levels(w, w, w)
+        args = (pp, dev_in(q), len(q), dev_out('resi', np.int16, (len(q), w, w)))
+        fn, exp = lib.vvb_inv_trquant_dev, dict(resi=inv_oracle(w, w, 0, 0, bd, qp, 0, q)[1])
+    else:
+        org, pred = org_pred_from(resi, bd)
+        args = (pp, dev_in(org), dev_in(pred), n, dev_out('q', np.int16, (n, w, w)), dev_out('reco', np.int16, (n, w, w)), dev_out('res', L.TU_RESULT_DT, (n,)),
+                dev_out('need_rdoq', np.uint8, (n,)))
+        fn, exp = lib.vvb_tu_roundtrip_dev, rt_oracle(w, w, 0, 0, bd, qp, 1, org, pred)
+    torch.cuda.synchronize()
+
+    def call():
+        assert fn(h, *args) == 0, lib.vvb_last_error(h)
+        torch.cuda.synchronize()
+        return {k: np.frombuffer(t[off:off + nb].cpu().numpy().tobytes(), dt).reshape(shape) for k, (t, dt, shape, nb) in outs.items()}
+    return call, exp
+
+
+@pytest.mark.gpu
+def test_dev_buffers_8_byte_aligned(eng):
+    """_dev calls on square 8 / 16 / 32 / 64 TUs with the tensor engines switched on, every pool and output 8 bytes into its torch allocation (8- but not 16-byte
+    aligned): forward from a pool and from planes, inverse and round trip equal the same calls on 16-byte aligned buffers and the oracle.  The misaligned calls
+    run on the CUDA-core kernels, the aligned ones on the raw-byte engines (test_kernel_selection)."""
+    eng.set_tensor_transform(1)
+    for w in (8, 16, 32, 64):
+        for entry in DEV_ENTRIES:
+            got = {}
+            for off in (8, 0):
+                call, exp = dev_case(eng, w, entry, off)
+                got[off] = g = call()
+                what = (w, entry, off)
+                if entry == 'inv':
+                    assert np.array_equal(g['resi'], exp['resi']), what
+                elif entry == 'rt':
+                    assert_rt(g, exp, what)
+                else:
+                    assert_fwd(g, exp, what)
+            assert got[8].keys() == got[0].keys()
+            for k in got[0]:
+                assert np.array_equal(got[8][k], got[0][k]), (w, entry, k)
+
+
 # ---------------------------------------------------------------------------------------------------- admission
 @pytest.mark.gpu
 def test_admission(eng):
@@ -653,7 +745,9 @@ def test_admission(eng):
 # ---------------------------------------------------------------------------------------------------- which kernels run
 def kernel_selection_cases():
     """[(label, setup)] for tests/_kernel_selection_run.py: the square 8..64 limit cases run the raw-byte engines (fwd_trquant_tc2_kernel, inv_trquant_tc_kernel)
-    with vvb_set_tensor_transform on and the CUDA-core kernels with it off; 4 x 4, rectangular TUs and sign-bit hiding run the CUDA-core kernels either way"""
+    with vvb_set_tensor_transform on and the CUDA-core kernels with it off; 4 x 4, rectangular TUs and sign-bit hiding run the CUDA-core kernels either way; with
+    the tensor engines on, the _dev calls of test_dev_buffers_8_byte_aligned run the raw-byte engines on 16-byte aligned buffers and the CUDA-core kernels on
+    buffers 8 bytes off"""
     from test_gpu_format_limits import ran
     cases = []
     for (w, h, sh) in ((8, 8, 0), (16, 16, 0), (32, 32, 0), (64, 64, 0), (4, 4, 0), (64, 4, 0), (16, 16, 1)):
@@ -676,6 +770,19 @@ def kernel_selection_cases():
                     other = {'fwd_trquant_tc2_kernel', 'inv_trquant_tc_kernel'} if not tc else set()
                     return call, (lambda names: all(ran(names, k) for k in want) and not any(ran(names, k) for k in other))
                 cases.append(('%dx%d sh=%d tensor=%d %s: %s' % (w, h, sh, tensor, entry, 'raw-byte engines' if tc else 'CUDA-core kernels'), setup))
+    for w in (8, 16, 32, 64):
+        for entry in DEV_ENTRIES:
+            for off in (0, 8):
+                tc = off == 0
+
+                def setup(eng, w=w, entry=entry, off=off, tc=tc):
+                    eng.set_tensor_transform(1)
+                    call, _ = dev_case(eng, w, entry, off)
+                    fwd_k, inv_k = ('fwd_trquant_tc2_kernel', 'inv_trquant_tc_kernel') if tc else ('fwd_trquant_kernel', 'inv_trquant_kernel')
+                    want = {'fwd': [fwd_k], 'fwd_planes': [fwd_k], 'inv': [inv_k], 'rt': [fwd_k, inv_k] if tc else ['tu_roundtrip_kernel']}[entry]
+                    other = {'fwd_trquant_tc2_kernel', 'inv_trquant_tc_kernel'} if not tc else set()
+                    return call, (lambda names: all(ran(names, k) for k in want) and not any(ran(names, k) for k in other))
+                cases.append(('%dx%d _dev %s buffers +%d bytes: %s' % (w, w, entry, off, 'raw-byte engines' if tc else 'CUDA-core kernels'), setup))
     return cases
 
 

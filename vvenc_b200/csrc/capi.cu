@@ -934,6 +934,23 @@ static int hadRingLaunch( vvb_ctx* ctx, const Plane& op, const Plane& rp, const 
   return VVB_OK;
 }
 
+// Dispatch of the TU kernels' compile-time shapes: f( std::integral_constant<int, LW>(), std::integral_constant<int, LH>() ) for the 25 shapes of
+// 2^lw x 2^lh (sides 4..64), f( std::integral_constant<int, N>() ) for the square sizes N = w of the tensor engines (8..64)
+template<int V> using IntC = std::integral_constant<int, V>;
+template<class F> static void forTuShape( int lw, int lh, F f )
+{
+  auto rows = [&]( auto LW ) {
+    switch( lh ) { case 2: f( LW, IntC<2>() ); break; case 3: f( LW, IntC<3>() ); break; case 4: f( LW, IntC<4>() ); break; case 5: f( LW, IntC<5>() ); break;
+                   default: f( LW, IntC<6>() ); break; }
+  };
+  switch( lw ) { case 2: rows( IntC<2>() ); break; case 3: rows( IntC<3>() ); break; case 4: rows( IntC<4>() ); break; case 5: rows( IntC<5>() ); break;
+                 default: rows( IntC<6>() ); break; }
+}
+template<class F> static void forSquare( int w, F f )
+{
+  switch( w ) { case 8: f( IntC<8>() ); break; case 16: f( IntC<16>() ); break; case 32: f( IntC<32>() ); break; default: f( IntC<64>() ); break; }
+}
+
 // B operand image of a tensor engine (table: vvb_ctx::tc2Image or itcImage) for the size and transform pair of p: build( std::integral_constant<int, N>, img )
 // fills it on the host at the first use, then it stays on the device
 template<class Build> static int bImage( vvb_ctx* ctx, const TuPar& p, void* ( &table )[36], const uint4** out, Build build )
@@ -942,8 +959,7 @@ template<class Build> static int bImage( vvb_ctx* ctx, const TuPar& p, void* ( &
   if( !slot )
   {
     std::vector<unsigned char> img;
-    switch( p.w ) { case 8: build( std::integral_constant<int, 8>(), img ); break; case 16: build( std::integral_constant<int, 16>(), img ); break;
-                    case 32: build( std::integral_constant<int, 32>(), img ); break; default: build( std::integral_constant<int, 64>(), img ); break; }
+    forSquare( p.w, [&]( auto N ) { build( N, img ); } );
     void* d = nullptr;
     CU( cudaMalloc( &d, img.size() ) );
     CU( cudaMemcpyAsync( d, img.data(), img.size(), cudaMemcpyHostToDevice, ctx->stream ) );
@@ -1160,7 +1176,6 @@ static int makeTuPar( vvb_ctx* ctx, const vvb_tu_par* in, TuPar& p )
   p.s2 = p.lh + 6;                                                                       // TrQuant.cpp:545
   if( p.s1 < 0 ) return fail( ctx, VVB_ERR_UNSUPPORTED, "negative first-stage shift (TrQuant.cpp:546 CHECK)" );
   p.offH = vvc_tr_offset_host[p.trHor][p.lw]; p.offV = vvc_tr_offset_host[p.trVer][p.lh];
-  p.regionW = std::min( 32, w ); p.regionH = std::min( 32, h );
   p.scanOff = ( ( p.lw - 2 ) * 5 + ( p.lh - 2 ) ) * 1024;
   p.ts = in->transform_skip ? 1 : 0;
   if( p.ts )
@@ -1193,19 +1208,21 @@ static int makeTuPar( vvb_ctx* ctx, const vvb_tu_par* in, TuPar& p )
   const int thrVal = 8;                                                                  // vvencCfg.cpp:971-973
   const int32_t thres = (int32_t)( (int64_t) thrVal << ( p.qbits - 1 ) );               // Quant.cpp:175-176 (TCoeff cast)
   p.useThres = thres / ( p.scale << 2 );                                                 // Quant.cpp:180
-  int t = ( w * h ) / 4;
-  p.team = std::max( 4, std::min( 128, t ) );
   {                                                                                      // Quant::dequant, Quant.cpp:554-607
-    const int qp = baseQpOf( p.ts != 0 ), per = qp / 6, rem = qp % 6;
     static const int invScales[2][6] = { { 40, 45, 51, 57, 64, 72 }, { 57, 64, 72, 80, 90, 102 } };   // g_invQuantScales, Rom.cpp:1396-1400
+    const int qp = baseQpOf( p.ts != 0 ), per = qp / 6, rem = qp % 6;
     p.dqScale = invScales[sqrt2][rem];
     p.dqShift = 6 - ( ( p.ts ? 0 : trShift ) + per );                                    // IQUANT_SHIFT = 6 (CommonDef.h:370); :561
+    // DepQuant::dequant (DepQuant.cpp:1492-1514 -> Quantizer::dequantBlock :574-629) at QP + 1 with one more bit of shift; skipped transforms never take it
+    const int qpDq = baseQpOf( false ) + 1, perDq = qpDq / 6;
+    p.dqDepScale = invScales[sqrt2][qpDq - 6 * perDq];
+    p.dqDepShift = 6 + 1 - perDq - trShift;
     const int tib = std::min( 16, 32 + p.dqShift - 7 );                                  // targetInputBitDepth, Quant.cpp:606
     p.dqInMax = ( 1 << ( tib - 1 ) ) - 1;
     p.s2Inv   = 20 - in->bit_depth;                                                      // TrQuant.cpp:609
     p.pelMax  = ( 1 << in->bit_depth ) - 1;
   }
-  p.lKeepW = ilog2h( p.keepW ); p.lKeepH = ilog2h( p.keepH ); p.lRegW = ilog2h( p.regionW );
+  p.lKeepW = ilog2h( p.keepW ); p.lKeepH = ilog2h( p.keepH );
   p.signHiding = in->sign_hiding ? 1 : 0;
   p.lfnstIdx = 0; p.lfnstTranspose = 0; p.lfnstMat = nullptr; p.lfnstMaxScan = 0x7fffffff;
   if( in->lfnst_idx )
@@ -1228,57 +1245,107 @@ static int makeTuPar( vvb_ctx* ctx, const vvb_tu_par* in, TuPar& p )
   return VVB_OK;
 }
 
-// forward tensor-core engine (trquant_tc2_kernels.cuh): square TUs 8..64 with the plain quantiser
-static bool tc2Eligible( const vvb_ctx* ctx, const TuPar& p )
+// The residual of a forward or round-trip call, one of the three sources of fwd_trquant_tc2_kernel's MODE (ResiMode): RESI_POOL one pool `resi`;
+// RESI_TWO_POOLS the original pool `resi` minus the prediction pool `pred`; RESI_PLANES the TU positions `blocks` in the two resident planes
+struct ResiSrc
 {
-  return ctx->tensorTransform && !p.lfnstIdx && !p.ts && !p.signHiding && p.w == p.h && p.w >= 8 && p.w <= 64 && p.s1 >= 0;
+  const int16_t* resi; const int16_t* pred; int orgPlane, predPlane; const vvb_block* blocks;
+  int mode() const { return blocks ? RESI_PLANES : pred ? RESI_TWO_POOLS : RESI_POOL; }
+};
+
+// Engine choice of the TU calls, one rule per direction.  The tensor engines read and write the residual and prediction pools, levels, coefficients,
+// residuals and reconstructions in 16-byte units, so besides the shape rule each needs every such buffer of the call (null ones aside) 16-byte aligned;
+// the CUDA-core kernels need no more than the element alignment.  Both engines are bit-exact.
+static bool aligned16( std::initializer_list<const void*> bufs )
+{
+  uintptr_t a = 0;
+  for( const void* b : bufs ) a |= (uintptr_t) b;
+  return ( a & 15 ) == 0;
 }
-// dResi alone: residual pool; dResi + dResi2: original and prediction pools; dBlocks: positions in the two planes
-static int tc2Launch( vvb_ctx* ctx, const TuPar& p, const int16_t* dResi, int orgPlane, int predPlane, const vvb_block* dBlocks, int n,
-                      int32_t* dCoef, int16_t* dQ, int32_t* dAbsSum, int32_t* dLastPos, uint8_t* dNeedRdoq, const int16_t* dResi2 = nullptr )
+// forward (fwd_trquant_tc2_kernel, trquant_tc2_kernels.cuh): square TUs 8..64 with the plain quantiser
+static bool tensorFwd( const vvb_ctx* ctx, const TuPar& p, bool aligned )
 {
-  const Plane po = dBlocks ? ctx->planes.p[orgPlane] : Plane{}, pp = dBlocks ? ctx->planes.p[predPlane] : Plane{};
+  return aligned && ctx->tensorTransform && !p.lfnstIdx && !p.ts && !p.signHiding && p.w == p.h && p.w >= 8 && p.w <= 64 && p.s1 >= 0;
+}
+// inverse (inv_trquant_tc_kernel, itrquant_tc_kernels.cuh): square TUs 8..64 without LFNST or transform skip, plain or DepQuant dequantiser parameters in p
+static bool tensorInv( const vvb_ctx* ctx, const TuPar& p, bool aligned )
+{
+  return aligned && ctx->tensorTransform && !p.lfnstIdx && !p.ts && p.w == p.h && p.w >= 8 && p.w <= 64;
+}
+// EXT instantiation of the CUDA-core forward and round-trip kernels: the plain one carries neither the LFNST stage, the sign-bit hiding pass nor transform skip
+static bool tuExt( const TuPar& p ) { return p.lfnstIdx != 0 || p.signHiding != 0 || p.ts != 0; }
+
+// CTAs per SM of kernel = fwd_trquant_tc2_kernel<N, mode> (dynamic shared memory smem) from its registers and shared memory, looked up at its first launch
+static int tc2PerSm( const void* kernel, int N, int mode, int smem )
+{
+  static int perSm[4][3] = {};
+  int& ps = perSm[ilog2h( N ) - 3][mode];
+  if( !ps )
+  {
+    cudaFuncAttributes fa = {};
+    cudaFuncGetAttributes( &fa, kernel );
+    const int regs = std::max( fa.numRegs, 32 );
+    ps = std::min( 65536 / ( regs * 128 ), ( 227 * 1024 ) / ( smem + (int) fa.sharedSizeBytes + 1024 ) );
+    ps = std::max( std::min( ps, N == 8 ? 6 : 8 ), 1 );
+  }
+  return ps;
+}
+
+static int tc2Launch( vvb_ctx* ctx, const TuPar& p, const ResiSrc& src, int n, int32_t* dCoef, int16_t* dQ, int32_t* dAbsSum, int32_t* dLastPos, uint8_t* dNeedRdoq )
+{
+  const Plane po = src.blocks ? ctx->planes.p[src.orgPlane] : Plane{}, pp = src.blocks ? ctx->planes.p[src.predPlane] : Plane{};
   const uint4* dImg; int rc;
   if( ( rc = bImage( ctx, p, ctx->tc2Image, &dImg, [&]( auto nc, std::vector<unsigned char>& img ) {
           constexpr int N = decltype( nc )::value; using S = Tc2Shape<N>;
           img.resize( 2 * S::B1_BYTES + 3 * S::B2_BYTES ); tc2_build_b_image<N>( vvc_tr_table_host, p.offH, p.offV, p.keepW, p.keepH, img.data() ); } ) ) ) return rc;
-#define VVB_FWD_TC_CALL( Nv ) { using S = Tc2Shape<Nv>; const int tiles = ( n + S::TPT - 1 ) / S::TPT; \
-    static int perSm[3] = { 0, 0, 0 }; const int mode = dBlocks ? 1 : dResi2 ? 2 : 0; int& ps = perSm[mode]; \
-    if( !ps ) { cudaFuncAttributes fa = {}; \
-                if( mode == 1 ) cudaFuncGetAttributes( &fa, fwd_trquant_tc2_kernel<Nv, 1> ); else if( mode == 2 ) cudaFuncGetAttributes( &fa, fwd_trquant_tc2_kernel<Nv, 2> ); \
-                else cudaFuncGetAttributes( &fa, fwd_trquant_tc2_kernel<Nv, 0> ); \
-                const int regs = std::max( fa.numRegs, 32 ); \
-                ps = std::min( 65536 / ( regs * 128 ), ( 227 * 1024 ) / ( (int) S::SMEM + (int) fa.sharedSizeBytes + 1024 ) ); ps = std::max( std::min( ps, Nv == 8 ? 6 : 8 ), 1 ); } \
-    const int grid = std::min( tiles, ctx->numSMs * ps ); \
-    if( mode == 1 )      fwd_trquant_tc2_kernel<Nv, 1><<<grid, 128, S::SMEM, ctx->stream>>>( p, dImg, ctx->d_scan, nullptr, nullptr, po, pp, dBlocks, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq ); \
-    else if( mode == 2 ) fwd_trquant_tc2_kernel<Nv, 2><<<grid, 128, S::SMEM, ctx->stream>>>( p, dImg, ctx->d_scan, dResi, dResi2, po, pp, nullptr, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq ); \
-    else                 fwd_trquant_tc2_kernel<Nv, 0><<<grid, 128, S::SMEM, ctx->stream>>>( p, dImg, ctx->d_scan, dResi, nullptr, po, pp, nullptr, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq ); }
-  switch( p.w ) { case 8: VVB_FWD_TC_CALL( 8 ) break; case 16: VVB_FWD_TC_CALL( 16 ) break; case 32: VVB_FWD_TC_CALL( 32 ) break; default: VVB_FWD_TC_CALL( 64 ) break; }
-#undef VVB_FWD_TC_CALL
+  forSquare( p.w, [&]( auto nc ) {
+    constexpr int N = decltype( nc )::value; using S = Tc2Shape<N>;
+    const int mode = src.mode();
+    const auto kernel = mode == RESI_PLANES ? fwd_trquant_tc2_kernel<N, RESI_PLANES> : mode == RESI_TWO_POOLS ? fwd_trquant_tc2_kernel<N, RESI_TWO_POOLS>
+                                                                                                         : fwd_trquant_tc2_kernel<N, RESI_POOL>;
+    const int grid = std::min( ( n + S::TPT - 1 ) / S::TPT, ctx->numSMs * tc2PerSm( (const void*) kernel, N, mode, (int) S::SMEM ) );
+    kernel<<<grid, 128, S::SMEM, ctx->stream>>>( p, dImg, ctx->d_scan, src.resi, src.pred, po, pp, src.blocks, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq );
+  } );
   CHECK_LAUNCH( "fwd_trquant_tc2_kernel" );
   return VVB_OK;
 }
 
-// inverse tensor-core engine (itrquant_tc_kernels.cuh): square 8 / 16 / 32 TUs, plain or DepQuant dequantiser parameters in p, no LFNST / transform skip
-static bool itcEligible( const vvb_ctx* ctx, const TuPar& p, const void* dQ )
-{
-  return ctx->tensorTransform && !p.lfnstIdx && !p.ts && p.w == p.h && p.w >= 8 && p.w <= 64 && ( ( (uintptr_t) dQ ) & 15 ) == 0;
-}
-// dResi != nullptr: levels -> residual.  Otherwise the second half of the TU round trip (reconstruction + distortions; dSum / dLast from the forward engine)
+// dResi != nullptr: levels -> residual.  Otherwise the second half of the TU round trip on the residual source src (reconstruction + distortions; dSum / dLast
+// from the forward engine)
 static int itcLaunch( vvb_ctx* ctx, const TuPar& p, const int16_t* dQ, int n, int16_t* dResi,
-                      int orgPlane, int predPlane, const vvb_block* dBlocks, const int16_t* dOrg, const int16_t* dPred, int16_t* dReco, TuResult* dRes, const int32_t* dSum, const int32_t* dLast )
+                      const ResiSrc& src, int16_t* dReco, TuResult* dRes, const int32_t* dSum, const int32_t* dLast )
 {
   const uint4* dImg; int rc;
   if( ( rc = bImage( ctx, p, ctx->itcImage, &dImg, [&]( auto nc, std::vector<unsigned char>& img ) {
           constexpr int N = decltype( nc )::value;
           img.resize( 4 * ItcShape<N>::B_BYTES ); itc_build_b_image<N>( vvc_tr_table_host, p.offH, p.offV, p.keepW, p.keepH, img.data() ); } ) ) ) return rc;
-  const Plane po = dBlocks ? ctx->planes.p[orgPlane] : Plane{}, pp = dBlocks ? ctx->planes.p[predPlane] : Plane{};
-#define VVB_ITC_CALL( Nv ) { using S = ItcShape<Nv>; const int tiles = ( n + S::TPT - 1 ) / S::TPT; const int grid = std::min( tiles, ctx->numSMs * std::min( 6, ( 227 * 1024 ) / ( S::SMEM + 1024 ) ) ); \
-    if( dResi ) inv_trquant_tc_kernel<Nv, false><<<grid, 128, S::SMEM, ctx->stream>>>( p, dImg, dQ, n, dResi, 0, po, pp, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr ); \
-    else        inv_trquant_tc_kernel<Nv, true><<<grid, 128, S::SMEM, ctx->stream>>>( p, dImg, dQ, n, nullptr, dBlocks ? 1 : 0, po, pp, dBlocks, dOrg, dPred, dReco, dRes, dSum, dLast ); }
-  switch( p.w ) { case 8: VVB_ITC_CALL( 8 ) break; case 16: VVB_ITC_CALL( 16 ) break; case 32: VVB_ITC_CALL( 32 ) break; default: VVB_ITC_CALL( 64 ) break; }
-#undef VVB_ITC_CALL
+  const Plane po = src.blocks ? ctx->planes.p[src.orgPlane] : Plane{}, pp = src.blocks ? ctx->planes.p[src.predPlane] : Plane{};
+  forSquare( p.w, [&]( auto nc ) {
+    constexpr int N = decltype( nc )::value; using S = ItcShape<N>;
+    const int grid = std::min( ( n + S::TPT - 1 ) / S::TPT, ctx->numSMs * std::min( 6, ( 227 * 1024 ) / ( S::SMEM + 1024 ) ) );
+    if( dResi ) inv_trquant_tc_kernel<N, false><<<grid, 128, S::SMEM, ctx->stream>>>( p, dImg, dQ, n, dResi, 0, po, pp, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr );
+    else        inv_trquant_tc_kernel<N, true><<<grid, 128, S::SMEM, ctx->stream>>>( p, dImg, dQ, n, nullptr, src.blocks ? 1 : 0, po, pp, src.blocks, src.resi, src.pred,
+                                                                                     dReco, dRes, dSum, dLast );
+  } );
   CHECK_LAUNCH( "inv_trquant_tc_kernel" );
+  return VVB_OK;
+}
+
+// forward transform + quantiser of n TUs (n > 0) from a pool (RESI_POOL) or from planes (RESI_PLANES)
+static int fwdLaunch( vvb_ctx* ctx, const TuPar& p, const ResiSrc& src, int n, int32_t* dCoef, int16_t* dQ, int32_t* dAbsSum, int32_t* dLastPos, uint8_t* dNeedRdoq )
+{
+  if( tensorFwd( ctx, p, aligned16( { src.resi, dCoef, dQ } ) ) ) return tc2Launch( ctx, p, src, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq );
+  // CUDA-core engine: planes form the residual while the TU is loaded (one launch, no compact residual buffer)
+  const Plane po = src.blocks ? ctx->planes.p[src.orgPlane] : Plane{}, pp = src.blocks ? ctx->planes.p[src.predPlane] : Plane{};
+  const bool ext = tuExt( p ), planes = src.blocks != nullptr;
+  forTuShape( p.lw, p.lh, [&]( auto lw, auto lh ) {
+    constexpr int LW = decltype( lw )::value, LH = decltype( lh )::value; using S = TuShape<LW, LH>;
+    const size_t smem = (size_t)( S::MAT_WORDS + S::NTEAMS * S::TEAM_WORDS ) * 4;
+    const auto kernel = ext ? ( planes ? fwd_trquant_kernel<LW, LH, true, RESI_PLANES> : fwd_trquant_kernel<LW, LH, true, RESI_POOL> )
+                            : ( planes ? fwd_trquant_kernel<LW, LH, false, RESI_PLANES> : fwd_trquant_kernel<LW, LH, false, RESI_POOL> );
+    kernel<<<teamGrid( ctx, n, S::NTEAMS, smem ), 128, smem, ctx->stream>>>( p, ctx->d_trTable, ctx->d_scan, src.resi, po, pp, src.blocks, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq );
+  } );
+  CHECK_LAUNCH( "fwd_trquant_kernel" );
   return VVB_OK;
 }
 
@@ -1290,15 +1357,7 @@ int vvb_fwd_trquant_dev( vvb_ctx* ctx, const vvb_tu_par* par, const int16_t* dRe
   if( rc ) return rc;
   if( n == 0 ) return VVB_OK;
   CU( cudaSetDevice( ctx->device ) );
-  if( tc2Eligible( ctx, p ) ) return tc2Launch( ctx, p, dResi, 0, 0, nullptr, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq );
-  const bool ext = p.lfnstIdx != 0 || p.signHiding != 0 || p.ts != 0;        // the plain instantiation carries neither the LFNST stage, the sign-bit hiding pass nor transform skip
-#define VVB_FWD_CALL( LWv, LHv ) { using S = TuShape<LWv, LHv>; const size_t smem = (size_t)( S::MAT_WORDS + S::NTEAMS * S::TEAM_WORDS ) * 4; \
-    if( ext ) fwd_trquant_kernel<LWv, LHv, true><<<teamGrid( ctx, n, S::NTEAMS, smem ), 128, smem, ctx->stream>>>( p, ctx->d_trTable, ctx->d_scan, dResi, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq ); \
-    else      fwd_trquant_kernel<LWv, LHv, false><<<teamGrid( ctx, n, S::NTEAMS, smem ), 128, smem, ctx->stream>>>( p, ctx->d_trTable, ctx->d_scan, dResi, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq ); }
-  VVB_TU_DISPATCH( p.lw, p.lh, VVB_FWD_CALL )
-#undef VVB_FWD_CALL
-  CHECK_LAUNCH( "fwd_trquant_kernel" );
-  return VVB_OK;
+  return fwdLaunch( ctx, p, ResiSrc{ dResi, nullptr, -1, -1, nullptr }, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq );
 }
 
 int vvb_fwd_trquant( vvb_ctx* ctx, const vvb_tu_par* par, const int16_t* resi, int n, int32_t* coef, int16_t* q, int32_t* absSum, int32_t* lastPos, uint8_t* needRdoq )
@@ -1321,17 +1380,7 @@ int vvb_fwd_trquant_planes_dev( vvb_ctx* ctx, const vvb_tu_par* par, int orgPlan
   TuPar p;
   int rc = makeTuPar( ctx, par, p );
   if( rc ) return rc;
-  if( tc2Eligible( ctx, p ) ) return tc2Launch( ctx, p, nullptr, orgPlane, predPlane, dBlocks, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq );
-  // CUDA-core engine: the residual is formed while the TU is loaded (one launch, no compact residual buffer)
-  const Plane &po = ctx->planes.p[orgPlane], &pp = ctx->planes.p[predPlane];
-  const bool ext = p.lfnstIdx != 0 || p.signHiding != 0 || p.ts != 0;
-#define VVB_FWDP_CALL( LWv, LHv ) { using S = TuShape<LWv, LHv>; const size_t smem = (size_t)( S::MAT_WORDS + S::NTEAMS * S::TEAM_WORDS ) * 4; \
-    if( ext ) fwd_trquant_planes_kernel<LWv, LHv, true><<<teamGrid( ctx, n, S::NTEAMS, smem ), 128, smem, ctx->stream>>>( p, ctx->d_trTable, ctx->d_scan, po, pp, dBlocks, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq ); \
-    else      fwd_trquant_planes_kernel<LWv, LHv, false><<<teamGrid( ctx, n, S::NTEAMS, smem ), 128, smem, ctx->stream>>>( p, ctx->d_trTable, ctx->d_scan, po, pp, dBlocks, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq ); }
-  VVB_TU_DISPATCH( p.lw, p.lh, VVB_FWDP_CALL )
-#undef VVB_FWDP_CALL
-  CHECK_LAUNCH( "fwd_trquant_planes_kernel" );
-  return VVB_OK;
+  return fwdLaunch( ctx, p, ResiSrc{ nullptr, nullptr, orgPlane, predPlane, dBlocks }, n, dCoef, dQ, dAbsSum, dLastPos, dNeedRdoq );
 }
 
 int vvb_fwd_trquant_planes( vvb_ctx* ctx, const vvb_tu_par* par, int orgPlane, int predPlane, const vvb_block* blocks, int n,
@@ -1689,6 +1738,35 @@ int vvb_rdoq_constants( const vvb_tu_par* par, const vvb_rdoq_par* rq, int32_t o
 }
 
 // ---- inverse path + fused TU round trip ------------------------------------------------------------------------------
+// dequantiser + inverse transform of n levels blocks (n > 0)
+static int invLaunch( vvb_ctx* ctx, const vvb_tu_par* par, TuPar p, const int16_t* dQ, int n, int16_t* dResi )
+{
+  const bool tensor = tensorInv( ctx, p, aligned16( { dQ, dResi } ) );
+  if( par->dep_quant && !p.ts )
+  {
+    // DepQuant::dequant (DepQuant.cpp:1492-1514 -> Quantizer::dequantBlock :574-629): the state machine turns the levels into qIdx values (up to +-65535) and
+    // dequantises them with the DepQuant scale and shift at QP + 1; the inverse kernel then reads the clipped coefficients with an identity dequantiser
+    void* dCoef;
+    int rc;
+    if( ( rc = scratch( ctx, ScratchArena::Work, (size_t) n * p.w * p.h * 2, &dCoef ) ) ) return rc;
+    const int lrw = std::min( p.lw, 5 ), nScan = std::min( p.w, 32 ) * std::min( p.h, 32 );
+    dq_dequant_levels_kernel<<<( n + 3 ) / 4, 128, 0, ctx->stream>>>( dQ, scanOrder( ctx->d_scan, p.lw, p.lh ), p.w, p.h, lrw, nScan, n, p.dqDepScale, p.dqDepShift,
+                                                                      (int16_t*) dCoef );
+    CHECK_LAUNCH( "dq_dequant_levels_kernel" );
+    p.dqScale = 1; p.dqShift = 0; p.dqInMax = 32767;
+    dQ = (const int16_t*) dCoef;
+  }
+  if( tensor ) return itcLaunch( ctx, p, dQ, n, dResi, ResiSrc{}, nullptr, nullptr, nullptr, nullptr );
+  forTuShape( p.lw, p.lh, [&]( auto lw, auto lh ) {
+    constexpr int LW = decltype( lw )::value, LH = decltype( lh )::value; using S = TuShape<LW, LH>;
+    const size_t smem = inv_trquant_smem<LW, LH>();
+    const auto kernel = p.lfnstIdx ? inv_trquant_kernel<LW, LH, true> : inv_trquant_kernel<LW, LH, false>;
+    kernel<<<teamGrid( ctx, n, S::NTEAMS, smem ), 128, smem, ctx->stream>>>( p, ctx->d_trTable, ctx->d_scan, dQ, n, dResi );
+  } );
+  CHECK_LAUNCH( "inv_trquant_kernel" );
+  return VVB_OK;
+}
+
 int vvb_inv_trquant_dev( vvb_ctx* ctx, const vvb_tu_par* par, const int16_t* dQ, int n, int16_t* dResi )
 {
   if( !ctx || !dQ || !dResi || n < 0 ) return fail( ctx, VVB_ERR_ARG, "bad arguments" );
@@ -1697,31 +1775,7 @@ int vvb_inv_trquant_dev( vvb_ctx* ctx, const vvb_tu_par* par, const int16_t* dQ,
   if( rc ) return rc;
   if( n == 0 ) return VVB_OK;
   CU( cudaSetDevice( ctx->device ) );
-  if( par->dep_quant && !p.ts )
-  {
-    // DepQuant::dequant (DepQuant.cpp:1492-1514 -> Quantizer::dequantBlock :574-629): the state machine turns the levels into qIdx values (up to +-65535) and
-    // dequantises them with the DepQuant scale and shift at QP + 1; the inverse kernel then reads the clipped coefficients with an identity dequantiser
-    const int qp = baseQp( par ) + 1;
-    const int per = qp / 6, rem = qp - 6 * per, sqrt2 = ( p.lw + p.lh ) & 1;
-    const int trShift = 15 - par->bit_depth - ( ( p.lw + p.lh ) >> 1 ) - sqrt2;
-    static const int invScales[2][6] = { { 40, 45, 51, 57, 64, 72 }, { 57, 64, 72, 80, 90, 102 } };
-    void* dCoef;
-    if( ( rc = scratch( ctx, ScratchArena::Work, (size_t) n * p.w * p.h * 2, &dCoef ) ) ) return rc;
-    const int lrw = std::min( p.lw, 5 ), nScan = std::min( p.w, 32 ) * std::min( p.h, 32 );
-    dq_dequant_levels_kernel<<<( n + 3 ) / 4, 128, 0, ctx->stream>>>( dQ, scanOrder( ctx->d_scan, p.lw, p.lh ), p.w, p.h, lrw, nScan, n, invScales[sqrt2][rem],
-                                                                      6 + 1 - per - trShift, (int16_t*) dCoef );
-    CHECK_LAUNCH( "dq_dequant_levels_kernel" );
-    p.dqScale = 1; p.dqShift = 0; p.dqInMax = 32767;
-    dQ = (const int16_t*) dCoef;
-  }
-  if( itcEligible( ctx, p, dQ ) && ( ( (uintptr_t) dResi ) & 15 ) == 0 ) return itcLaunch( ctx, p, dQ, n, dResi, 0, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr );
-#define VVB_INV_CALL( LWv, LHv ) { using S = TuShape<LWv, LHv>; const size_t smem = inv_trquant_smem<LWv, LHv>(); \
-    if( p.lfnstIdx ) inv_trquant_kernel<LWv, LHv, true><<<teamGrid( ctx, n, S::NTEAMS, smem ), 128, smem, ctx->stream>>>( p, ctx->d_trTable, ctx->d_scan, dQ, n, dResi ); \
-    else             inv_trquant_kernel<LWv, LHv, false><<<teamGrid( ctx, n, S::NTEAMS, smem ), 128, smem, ctx->stream>>>( p, ctx->d_trTable, ctx->d_scan, dQ, n, dResi ); }
-  VVB_TU_DISPATCH( p.lw, p.lh, VVB_INV_CALL )
-#undef VVB_INV_CALL
-  CHECK_LAUNCH( "inv_trquant_kernel" );
-  return VVB_OK;
+  return invLaunch( ctx, par, p, dQ, n, dResi );
 }
 
 int vvb_inv_trquant( vvb_ctx* ctx, const vvb_tu_par* par, const int16_t* q, int n, int16_t* resi )
@@ -1735,39 +1789,32 @@ int vvb_inv_trquant( vvb_ctx* ctx, const vvb_tu_par* par, const int16_t* q, int 
 
 static_assert( sizeof( vvb_tu_result ) == sizeof( TuResult ) && sizeof( TuResult ) == 32, "vvb_tu_result layout" );
 
-static int tuRoundtripLaunch( vvb_ctx* ctx, const vvb_tu_par* par, int orgPlane, int predPlane, const vvb_block* dBlocks, const int16_t* dOrg, const int16_t* dPred,
-                              int n, int16_t* dQ, int16_t* dReco, vvb_tu_result* dRes, uint8_t* dNeedRdoq )
+// fused round trip of n TUs: the tensor pair (forward engine for the levels, absSum, lastPos and RDOQ flag, then the inverse engine from the levels) where
+// both directions take the call, tu_roundtrip_kernel otherwise
+static int rtLaunch( vvb_ctx* ctx, const vvb_tu_par* par, const ResiSrc& src, int n, int16_t* dQ, int16_t* dReco, vvb_tu_result* dRes, uint8_t* dNeedRdoq )
 {
   TuPar p;
   int rc = makeTuPar( ctx, par, p );
   if( rc ) return rc;
   if( n == 0 ) return VVB_OK;
   CU( cudaSetDevice( ctx->device ) );
-  const Plane po = dBlocks ? ctx->planes.p[orgPlane] : Plane{}, pp = dBlocks ? ctx->planes.p[predPlane] : Plane{};
-  const bool ext = p.signHiding != 0 || p.ts != 0 || p.lfnstIdx != 0;
-  // square 8..64 TUs with the plain quantiser: the forward half on the tensor-core engine (levels, absSum, lastPos, RDOQ flag), then the inverse half from the levels
-  if( tc2Eligible( ctx, p ) && ( dBlocks || ( ( ( (uintptr_t) dOrg | (uintptr_t) dPred ) & 15 ) == 0 ) ) )
+  const bool aligned = aligned16( { src.resi, src.pred, dQ, dReco } );
+  if( tensorFwd( ctx, p, aligned ) && tensorInv( ctx, p, aligned ) )
   {
     int32_t *dSum, *dLast;
     if( ( rc = carveArena( ctx, ScratchArena::Work, [&]( Layout& L ) { dSum = L.take<int32_t>( n ); dLast = L.take<int32_t>( n ); } ) ) ) return rc;
-    if( ( rc = tc2Launch( ctx, p, dBlocks ? nullptr : dOrg, orgPlane, predPlane, dBlocks, n, nullptr, dQ, dSum, dLast, dNeedRdoq, dBlocks ? nullptr : dPred ) ) ) return rc;
-    if( itcEligible( ctx, p, dQ ) && ( !dReco || ( ( (uintptr_t) dReco ) & 15 ) == 0 ) )
-      return itcLaunch( ctx, p, dQ, n, nullptr, orgPlane, predPlane, dBlocks, dOrg, dPred, dReco, (TuResult*) dRes, dSum, dLast );
-#define VVB_RTQ_CALL( LWv, LHv ) { using S = TuShape<LWv, LHv>; const size_t smem = tu_roundtrip_smem<LWv, LHv>(); \
-      tu_roundtrip_kernel<LWv, LHv, false, true><<<teamGrid( ctx, n, S::NTEAMS, smem ), 128, smem, ctx->stream>>>( p, ctx->d_trTable, ctx->d_scan, dBlocks ? 1 : 0, po, pp, dBlocks, dOrg, dPred, n, \
-                                                                                              dQ, dReco, (TuResult*) dRes, dNeedRdoq, dSum, dLast ); }
-    switch( p.lw ) { case 3: VVB_RTQ_CALL( 3, 3 ) break; case 4: VVB_RTQ_CALL( 4, 4 ) break; case 5: VVB_RTQ_CALL( 5, 5 ) break; default: VVB_RTQ_CALL( 6, 6 ) break; }
-#undef VVB_RTQ_CALL
-    CHECK_LAUNCH( "tu_roundtrip_kernel (from levels)" );
-    return VVB_OK;
+    if( ( rc = tc2Launch( ctx, p, src, n, nullptr, dQ, dSum, dLast, dNeedRdoq ) ) ) return rc;
+    return itcLaunch( ctx, p, dQ, n, nullptr, src, dReco, (TuResult*) dRes, dSum, dLast );
   }
-#define VVB_RT_CALL( LWv, LHv ) { using S = TuShape<LWv, LHv>; const size_t smem = tu_roundtrip_smem<LWv, LHv>(); \
-    if( ext ) tu_roundtrip_kernel<LWv, LHv, true><<<teamGrid( ctx, n, S::NTEAMS, smem ), 128, smem, ctx->stream>>>( p, ctx->d_trTable, ctx->d_scan, dBlocks ? 1 : 0, po, pp, dBlocks, dOrg, dPred, n, \
-                                                                                              dQ, dReco, (TuResult*) dRes, dNeedRdoq ); \
-    else      tu_roundtrip_kernel<LWv, LHv, false><<<teamGrid( ctx, n, S::NTEAMS, smem ), 128, smem, ctx->stream>>>( p, ctx->d_trTable, ctx->d_scan, dBlocks ? 1 : 0, po, pp, dBlocks, dOrg, dPred, n, \
-                                                                                              dQ, dReco, (TuResult*) dRes, dNeedRdoq ); }
-  VVB_TU_DISPATCH( p.lw, p.lh, VVB_RT_CALL )
-#undef VVB_RT_CALL
+  const Plane po = src.blocks ? ctx->planes.p[src.orgPlane] : Plane{}, pp = src.blocks ? ctx->planes.p[src.predPlane] : Plane{};
+  const bool ext = tuExt( p );
+  forTuShape( p.lw, p.lh, [&]( auto lw, auto lh ) {
+    constexpr int LW = decltype( lw )::value, LH = decltype( lh )::value; using S = TuShape<LW, LH>;
+    const size_t smem = tu_roundtrip_smem<LW, LH>();
+    const auto kernel = ext ? tu_roundtrip_kernel<LW, LH, true> : tu_roundtrip_kernel<LW, LH, false>;
+    kernel<<<teamGrid( ctx, n, S::NTEAMS, smem ), 128, smem, ctx->stream>>>( p, ctx->d_trTable, ctx->d_scan, src.blocks ? 1 : 0, po, pp, src.blocks, src.resi, src.pred, n,
+                                                                            dQ, dReco, (TuResult*) dRes, dNeedRdoq );
+  } );
   CHECK_LAUNCH( "tu_roundtrip_kernel" );
   return VVB_OK;
 }
@@ -1775,7 +1822,7 @@ static int tuRoundtripLaunch( vvb_ctx* ctx, const vvb_tu_par* par, int orgPlane,
 int vvb_tu_roundtrip_dev( vvb_ctx* ctx, const vvb_tu_par* par, const int16_t* dOrg, const int16_t* dPred, int n, int16_t* dQ, int16_t* dReco, vvb_tu_result* dRes, uint8_t* dNeedRdoq )
 {
   if( !ctx || !dOrg || !dPred || !dQ || !dRes || n < 0 ) return fail( ctx, VVB_ERR_ARG, "bad arguments" );
-  return tuRoundtripLaunch( ctx, par, -1, -1, nullptr, dOrg, dPred, n, dQ, dReco, dRes, dNeedRdoq );
+  return rtLaunch( ctx, par, ResiSrc{ dOrg, dPred, -1, -1, nullptr }, n, dQ, dReco, dRes, dNeedRdoq );
 }
 
 int vvb_tu_roundtrip_planes_dev( vvb_ctx* ctx, const vvb_tu_par* par, int orgPlane, int predPlane, const vvb_block* dBlocks, int n,
@@ -1783,7 +1830,7 @@ int vvb_tu_roundtrip_planes_dev( vvb_ctx* ctx, const vvb_tu_par* par, int orgPla
 {
   if( !ctx || !dBlocks || !dQ || !dRes || n < 0 ) return fail( ctx, VVB_ERR_ARG, "bad arguments" );
   if( !validPlane( ctx, orgPlane ) || !validPlane( ctx, predPlane ) ) return fail( ctx, VVB_ERR_ARG, "unknown plane" );
-  return tuRoundtripLaunch( ctx, par, orgPlane, predPlane, dBlocks, nullptr, nullptr, n, dQ, dReco, dRes, dNeedRdoq );
+  return rtLaunch( ctx, par, ResiSrc{ nullptr, nullptr, orgPlane, predPlane, dBlocks }, n, dQ, dReco, dRes, dNeedRdoq );
 }
 
 int vvb_tu_roundtrip( vvb_ctx* ctx, const vvb_tu_par* par, const int16_t* org, const int16_t* pred, int n, int16_t* q, int16_t* reco, vvb_tu_result* res, uint8_t* needRdoq )

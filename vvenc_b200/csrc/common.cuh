@@ -87,7 +87,7 @@ struct vvb_ctx
   bool           poolBlocksAligned = false;   // see vvb_pool_hint
   void*          itcImage[36] = {};           // the same for the inverse tensor engine
   void*          tc2Image[36] = {};           // B operand images of the raw-byte tensor engine, index ((lw - 3) * 3 + trHor) * 3 + trVer
-  bool           tensorTransform = true;      // see vvb_set_tensor_transform: on = raw-byte wgmma engines where they apply (tc2Eligible, itcEligible), off = CUDA cores for every shape
+  bool           tensorTransform = true;      // see vvb_set_tensor_transform: on = raw-byte wgmma engines where they apply (tensorFwd, tensorInv in capi.cu), off = CUDA cores for every shape
   int            rdoqEngine = 1;              // see vvb_set_rdoq_engine: 1 = templates gathered per position (first engine, verified on hardware), 2 = accumulated templates + cost tables
   int            dqEngine = 1;                // see vvb_set_depquant_engine: 1 = four lanes per TU (one per trellis state), 0 = one thread per TU
   int            pyramidEngine = 1;           // see vvb_set_pyramid_engine: 1 = all pyramid levels inside one CTA per root block, 0 = per-quad kernel + table sums

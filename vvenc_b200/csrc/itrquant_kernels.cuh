@@ -330,13 +330,11 @@ template<int LW, int LH> static inline size_t tu_roundtrip_smem()
   return (size_t)( S::MAT_WORDS + I::MAT_WORDS + S::NTEAMS * ( S::TEAM_WORDS + 8 ) ) * 4;
 }
 
-// FROMQ: the forward half already ran (the tensor-core engine wrote levels, absSum, lastPos and the RDOQ flag): the kernel starts from the levels in qOut
-template<int LW, int LH, bool EXT, bool FROMQ = false>
+template<int LW, int LH, bool EXT>
 __global__ void __launch_bounds__( 128 ) tu_roundtrip_kernel( const __grid_constant__ TuPar par, const int8_t* __restrict__ trTable, const int32_t* __restrict__ scanTab,
                                                               const int planes, const __grid_constant__ Plane orgPlane, const __grid_constant__ Plane predPlane,
                                                               const vvb_block* __restrict__ blocks, const int16_t* __restrict__ orgPool, const int16_t* __restrict__ predPool, int n,
-                                                              int16_t* __restrict__ qOut, int16_t* __restrict__ recoOut, TuResult* __restrict__ resOut, uint8_t* __restrict__ needRdoqOut,
-                                                              const int32_t* __restrict__ absSumIn = nullptr, const int32_t* __restrict__ lastPosIn = nullptr )
+                                                              int16_t* __restrict__ qOut, int16_t* __restrict__ recoOut, TuResult* __restrict__ resOut, uint8_t* __restrict__ needRdoqOut )
 {
   using S = TuShape<LW, LH>; using I = InvShape<LW, LH>;
   extern __shared__ __align__( 16 ) uint32_t smem[];
@@ -347,11 +345,8 @@ __global__ void __launch_bounds__( 128 ) tu_roundtrip_kernel( const __grid_const
   uint32_t* MvI = smem + S::MAT_WORDS;
   uint32_t* MhI = MvI + ( S::RH / 4 ) * H;
   uint32_t* teamBase = MvI + I::MAT_WORDS;
-  if( !FROMQ )
-  {
-    stage_matrix( MtH, trTable, par.offH, W, par.keepW, S::RW, threadIdx.x, blockDim.x );
-    stage_matrix( MtV, trTable, par.offV, H, par.keepH, S::RH, threadIdx.x, blockDim.x );
-  }
+  stage_matrix( MtH, trTable, par.offH, W, par.keepW, S::RW, threadIdx.x, blockDim.x );
+  stage_matrix( MtV, trTable, par.offV, H, par.keepH, S::RH, threadIdx.x, blockDim.x );
   stage_matrix_inv( MvI, trTable, par.offV, H, par.keepH, S::RH / 4, threadIdx.x, blockDim.x );
   stage_matrix_inv( MhI, trTable, par.offH, W, par.keepW, S::RW / 4, threadIdx.x, blockDim.x );
   const TeamView v = team_view<S>( teamBase, team );
@@ -373,35 +368,14 @@ __global__ void __launch_bounds__( 128 ) tu_roundtrip_kernel( const __grid_const
       oBase = orgPool + (size_t)( live ? tu : 0 ) * W * H;   so = W;
       pBase = predPool + (size_t)( live ? tu : 0 ) * W * H;  sp = W;
     }
-    const bool al4 = ( ( ( reinterpret_cast<uintptr_t>( oBase ) | reinterpret_cast<uintptr_t>( pBase ) ) & 3 ) | ( ( so | sp ) & 1 ) ) == 0;   // word loads allowed
     const bool al8 = ( ( ( reinterpret_cast<uintptr_t>( oBase ) | reinterpret_cast<uintptr_t>( pBase ) ) & 7 ) | ( ( so | sp ) & 3 ) ) == 0;   // 4-pel loads allowed
-    int pos, absSum, lastQ1;
-    if( FROMQ )
+    const int pos = team_forward<LW, LH, EXT>( par, MtH, MtV, v, scanTab, tt, live, org_pred_words<LW>( oBase, so, pBase, sp ) );
+    const int absSum = v.red[4], lastQ1 = v.red[5];
+    if( live )
     {
-      __syncthreads();                                        // the previous TU's inverse is done with the level block
-      const uint32_t* src = reinterpret_cast<const uint32_t*>( qOut + (size_t)( live ? tu : 0 ) * W * H );
+      uint32_t* dst = reinterpret_cast<uint32_t*>( qOut + (size_t) tu * W * H );
 #pragma unroll
-      for( int k = 0; k < S::RESI_WORDS / T; k++ ) if( live ) v.resi[tt + k * T] = src[tt + k * T];
-      absSum = live ? absSumIn[tu] : 0; pos = live ? lastPosIn[tu] : 0; lastQ1 = pos + 1;
-      __syncthreads();
-    }
-    else
-    {
-      pos = team_forward<LW, LH, EXT>( par, MtH, MtV, v, scanTab, tt, live, [&]( int i )
-      {
-        const int y = i >> ( LW - 1 ), x = ( i & ( W / 2 - 1 ) ) << 1;
-        const int16_t* o = oBase + (ptrdiff_t) y * so + x; const int16_t* p = pBase + (ptrdiff_t) y * sp + x;
-        if( al4 ) return __vsub2( __ldg( reinterpret_cast<const uint32_t*>( o ) ), __ldg( reinterpret_cast<const uint32_t*>( p ) ) );
-        const int d0 = (int) __ldg( o ) - (int) __ldg( p ), d1 = (int) __ldg( o + 1 ) - (int) __ldg( p + 1 );
-        return ( (uint32_t) d0 & 0xffffu ) | ( (uint32_t) d1 << 16 );
-      } );
-      absSum = v.red[4]; lastQ1 = v.red[5];
-      if( live )
-      {
-        uint32_t* dst = reinterpret_cast<uint32_t*>( qOut + (size_t) tu * W * H );
-#pragma unroll
-        for( int k = 0; k < S::RESI_WORDS / T; k++ ) dst[tt + k * T] = v.resi[tt + k * T];
-      }
+      for( int k = 0; k < S::RESI_WORDS / T; k++ ) dst[tt + k * T] = v.resi[tt + k * T];
     }
     // every thread has read absSum before any thread can pass the first barrier of team_inverse; red[] is only reset in the next team_forward
     const bool active = live && absSum > 0;
@@ -477,7 +451,7 @@ __global__ void __launch_bounds__( 128 ) tu_roundtrip_kernel( const __grid_const
       r.distReco = dReco; r.distResi = dResi; r.distZero = dZero;
       r.absSum = absSum; r.lastPos = absSum ? lastQ1 - 1 : pos;
       resOut[tu] = r;
-      if( !FROMQ && needRdoqOut ) needRdoqOut[tu] = (uint8_t) v.red[6];
+      if( needRdoqOut ) needRdoqOut[tu] = (uint8_t) v.red[6];
     }
   }
 }
