@@ -56,7 +56,7 @@ int         vvb_launch_count( const vvb_ctx* ctx, uint64_t* kernels_launched );
 int         vvb_set_async  ( vvb_ctx* ctx, int enable );   /* kernels this context has launched so far */
 
 /* measurement aid (bench.py): issue-rate probe of the packed-SAD instruction mix; no reference counterpart */
-int         vvb_alu_probe_dev( vvb_ctx* ctx, int grid_ctas, int iters, int mode /* 0: max-min SAD mix, 1: min-only mix of the dense search */ );
+int         vvb_alu_probe_dev( vvb_ctx* ctx, int grid_ctas, int iters, int mode /* 0: max-min SAD mix, 1: min-only mix of the dense search, 2: the SAD pyramid's tensor-core mix (min + relu + HMMA), 3: min + HMMA, 4: HMMA alone */ );
 
 /* ---- pictures ("planes") ---------------------------------------------------------------------------------
  * int16 sample planes (Pel, CommonLib/TypeDef.h:181) with a margin on all sides, like the encoder's padded

@@ -250,14 +250,51 @@ __global__ void fix_wsse_kernel( const int16_t* org, int so, const int16_t* cur,
   if( threadIdx.x == 0 ) *out = acc;
 }
 
-// Issue-rate probe for the packed-SAD instruction mix (2 x VIMNMX.S16x2 + 2 x IDP.2A per pel pair) on register operands:
-// the measured ceiling the dense search kernel is compared against (bench.py "alu" roofline).
+// A tensor-core formulation of the SAD pyramid's pel sums, timed by the probe below (modes 2..4) and used by no kernel (DESIGN §5 has the measurement that
+// kept it out of sad_pyramid8_kernel).  Pels biased to the fp16 number 1024 + v have the bit pattern
+// 0x6400 | v (v <= 1023), so VIMNMX.S16x2 on the bits is the biased minimum (|a - b| = a + b - 2 min(a, b)) and HFMA2.RELU (o * -1 + w) is max(b - a, 0)
+// (|a - b| = a - b + 2 max(b - a, 0)), both exact; one HMMA.16816.F32 against a fixed selector then sums, lane by lane, four such words into four fp32
+// accumulators.
+__device__ __forceinline__ uint32_t mma_relu_diff( uint32_t o, uint32_t w )
+{
+  uint32_t d;
+  asm( "fma.rn.relu.f16x2 %0, %1, %2, %3;" : "=r"( d ) : "r"( o ), "r"( 0xbc00bc00u ), "r"( w ) );
+  return d;
+}
+
+// Selector B (16 x 8): B[k][n] = -2 for even n, +2 for odd n, where n = (k & 6) + (k >> 3), else 0.  Lane (g = lane / 4, t = lane % 4) holds
+// {B[2t][g], B[2t+1][g]} and {B[2t+8][g], B[2t+9][g]}; D[g][2t] then sums only the lane's own A[g][2t..2t+1], and so on for the other three accumulators.
+__device__ __forceinline__ void mma_selector( int lane, uint32_t (&b)[2] )
+{
+  const int g = lane >> 2, t = lane & 3;
+  b[0] = g == 2 * t ? 0xc000c000u : 0u;          // -2, -2
+  b[1] = g == 2 * t + 1 ? 0x40004000u : 0u;      // +2, +2
+}
+
+// c[0] -= 2 (m0.lo + m0.hi), c[1] -= 2 (m1.lo + m1.hi), c[2] += 2 (r0.lo + r0.hi), c[3] += 2 (r1.lo + r1.hi), every lane on its own registers
+__device__ __forceinline__ void mma_sum4( float (&c)[4], uint32_t m0, uint32_t m1, uint32_t r0, uint32_t r1, uint32_t b0, uint32_t b1 )
+{
+  asm( "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+       : "+f"( c[0] ), "+f"( c[2] ), "+f"( c[1] ), "+f"( c[3] ) : "r"( m0 ), "r"( m1 ), "r"( r0 ), "r"( r1 ), "r"( b0 ), "r"( b1 ) );
+}
+
+// Issue-rate probe for the packed-SAD instruction mixes on register operands: the measured ceiling the dense search kernel is compared against (bench.py
+// "alu" roofline).  Per iteration 8 packed words (16 pel differences): MODE 0 VIMNMX.S16x2 x 2 + IDP.2A x 2 per word, MODE 1 VIMNMX.S16x2 + IDP.2A per word,
+// MODE 2 the tensor-core mix of the SAD pyramid's pel sums (per 4 words: 2 VIMNMX.S16x2 + 2 HFMA2.RELU + 1 HMMA.16816.F32), MODE 3 the same with 4 VIMNMX.S16x2 and no HFMA2,
+// MODE 4 the HMMA alone.
 template<int MODE>
 __global__ void __launch_bounds__( 256 ) alu_probe_kernel( int iters, uint32_t seed, uint32_t* out )
 {
   uint32_t a[8], b[8]; int acc[8];
+  float cf[2][4] = {};
+  uint32_t bsel[2];
+  mma_selector( threadIdx.x & 31, bsel );
 #pragma unroll
-  for( int i = 0; i < 8; i++ ) { a[i] = seed * ( 2654435761u + i ) + threadIdx.x; b[i] = a[i] ^ ( 0x01230123u * ( i + 1 ) ); acc[i] = 0; }
+  for( int i = 0; i < 8; i++ )
+  {
+    a[i] = seed * ( 2654435761u + i ) + threadIdx.x; b[i] = a[i] ^ ( 0x01230123u * ( i + 1 ) ); acc[i] = 0;
+    if( MODE >= 2 ) { a[i] = ( a[i] & 0x03ff03ffu ) | 0x64006400u; b[i] = ( b[i] & 0x03ff03ffu ) | 0x64006400u; }     // biased pels
+  }
   for( int it = 0; it < iters; it++ )
   {
 #pragma unroll
@@ -271,17 +308,40 @@ __global__ void __launch_bounds__( 256 ) alu_probe_kernel( int iters, uint32_t s
         acc[i] = __dp2a_lo( (int) mn, (int) 0x0000ffffu, acc[i] );
         a[i] = mx; b[i] = mn;
       }
-      else                 // dense search: only sum min(a,b) is per-candidate work
+      else if( MODE == 1 ) // dense search: only sum min(a,b) is per-candidate work
       {
         const uint32_t mn = __vmins2( a[i], b[i] );
         acc[i] = __dp2a_lo( (int) mn, (int) 0x0000ffffu, acc[i] );
         a[i] = b[i]; b[i] = mn;
       }
     }
+    if( MODE >= 2 )
+    {
+      // tensor-core pel sums (mma_sum4): 8 words = 2 HMMA steps of 4 words each.  MODE 2: two minima (alu pipe) + two HFMA2.RELU (fma pipe)
+      // per step; MODE 3: four minima, no HFMA2; MODE 4: the HMMA steps alone.  Step 1 turns words a into t, step 2 turns t back into a, so that no
+      // step overwrites the operands of the HMMA just issued and the compiler adds no copies.
+      if( MODE == 4 )
+      {
+        mma_sum4( cf[0], a[0], a[1], a[2], a[3], bsel[0], bsel[1] );
+        mma_sum4( cf[1], a[4], a[5], a[6], a[7], bsel[0], bsel[1] );
+      }
+      else
+      {
+        uint32_t t[4];
+#pragma unroll
+        for( int i = 0; i < 4; i++ ) t[i] = ( MODE == 3 || i < 2 ) ? __vmins2( a[i], b[i] ) : mma_relu_diff( b[i], a[i] );
+        mma_sum4( cf[0], t[0], t[1], t[2], t[3], bsel[0], bsel[1] );
+#pragma unroll
+        for( int i = 0; i < 4; i++ ) a[i] = ( MODE == 3 || i < 2 ) ? __vmins2( t[i], b[i + 4] ) : mma_relu_diff( b[i + 4], t[i] );
+        mma_sum4( cf[1], a[0], a[1], a[2], a[3], bsel[0], bsel[1] );
+      }
+    }
   }
   int s = 0;
 #pragma unroll
   for( int i = 0; i < 8; i++ ) s += acc[i];
+#pragma unroll
+  for( int j = 0; j < 2; j++ ) s += (int)( cf[j][0] + cf[j][1] + cf[j][2] + cf[j][3] );
   if( s == 0x7fffffff ) out[0] = (uint32_t) s;      // keeps the loop alive
 }
 
@@ -433,15 +493,18 @@ int vvb_set_tensor_transform( vvb_ctx* ctx, int enable )
   return VVB_OK;
 }
 
-// launches the ALU probe: grid_ctas CTAs x 256 threads x iters iterations x 8 packed SADs (16 pel differences) each
+// launches the ALU probe: grid_ctas CTAs x 256 threads x iters iterations x 8 packed words (16 pel differences) each
 int vvb_alu_probe_dev( vvb_ctx* ctx, int gridCtas, int iters, int mode )
 {
   if( !ctx || gridCtas < 1 || iters < 1 ) return fail( ctx, VVB_ERR_ARG, "bad arguments" );
   CU( cudaSetDevice( ctx->device ) );
   void* d; int rc;
   if( ( rc = scratch( ctx, ScratchArena::Work, 64, &d ) ) ) return rc;
-  if( mode == 0 ) alu_probe_kernel<0><<<gridCtas, 256, 0, ctx->stream>>>( iters, 12345u, (uint32_t*) d );
-  else            alu_probe_kernel<1><<<gridCtas, 256, 0, ctx->stream>>>( iters, 12345u, (uint32_t*) d );
+  if( mode == 0 )      alu_probe_kernel<0><<<gridCtas, 256, 0, ctx->stream>>>( iters, 12345u, (uint32_t*) d );
+  else if( mode == 2 ) alu_probe_kernel<2><<<gridCtas, 256, 0, ctx->stream>>>( iters, 12345u, (uint32_t*) d );
+  else if( mode == 3 ) alu_probe_kernel<3><<<gridCtas, 256, 0, ctx->stream>>>( iters, 12345u, (uint32_t*) d );
+  else if( mode == 4 ) alu_probe_kernel<4><<<gridCtas, 256, 0, ctx->stream>>>( iters, 12345u, (uint32_t*) d );
+  else                 alu_probe_kernel<1><<<gridCtas, 256, 0, ctx->stream>>>( iters, 12345u, (uint32_t*) d );
   CHECK_LAUNCH( "alu_probe_kernel" );
   return VVB_OK;
 }

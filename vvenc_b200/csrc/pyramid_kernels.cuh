@@ -7,16 +7,17 @@
 // four children's SADs in registers; 32x32 tables are accumulated in shared memory and the 64x64 table is their sum -- no cost table ever leaves the SM
 // (the previous design moved about 1.2 GB of 16x16 / 32x32 tables through HBM per 2160p picture).
 //
-// Arithmetic per (8x8 block, candidate):  SAD = sum a + sum b - 2 sum min(a,b)
-//   sum a : per block, once;  sum b : 8x8 box sums of the window (uint16 table V);  sum min : VIMNMX.S16x2 (alu pipe) + IDP.2A (fma pipe) per pel pair.
-// Both pipes accept a warp instruction every other cycle per scheduler, so one min + one dot product per pel pair is the floor of this
-// formulation; everything else is kept off the alu pipe where possible:
+// Arithmetic per (8x8 block, candidate):  SAD = sum a - sum b + 2 sum max(b - a, 0)
+//   sum a : per block, once;  sum b : 8x8 box sums of the window (uint16 table V);  sum max : HFMA2.RELU (fma pipe; pels up to 1023 are exact fp16
+//   subnormals) per pel pair, and per two pel pairs one IADD3 (alu pipe) into two uint16 lanes.  That is 1.5 instructions per pel pair where a min
+//   (VIMNMX.S16x2, alu) + dot product (IDP.2A, fma) took 2, and the alu pipe carries half an instruction per pair instead of one.  Everything else is kept
+//   off the alu pipe where possible:
 //   * odd-offset candidates read a second, one-pel-shifted copy of the window (no funnel shifts),
 //   * a thread evaluates TWO vertically adjacent candidate rows for a strip of 8 vectors: the nine window rows they need are loaded once (LDS.128) and
 //     every original row serves both (shared-memory traffic per candidate halves),
 //   * the epilogue per candidate is IDP.4A (shared address of the rate entry: table base + row bits, plus column bits), LDS (rate table pre-multiplied
-//     by 8, one table per strip slot so that the slot index is part of the entry), IDP.2A (unpack the box sum and add it), IMAD (parent sum), IMAD (key)
-//     on the fma pipe and half a VIMNMX3.
+//     by 8, one table per strip slot so that the slot index is part of the entry), IDP.2A (sum a + 2 * the two uint16 lanes), IDP.2A (unpack the box sum
+//     and subtract it), IMAD (parent sum), IMAD (key) on the fma pipe and half a VIMNMX3.
 //   * strip slots past the end of the range carry MV-bit count 250 and read rate-table entries that can never win; no predicate per candidate.
 //   * the item keeps its base addresses and the four members step through fixed offsets.  For 32x32 and 64x64 roots the CTA has at most 512 threads so
 //     that ptxas may keep them in 128 registers (at 640 threads the 96-register cap forced their recomputation in every member).
@@ -119,8 +120,20 @@ __device__ __forceinline__ void pyr_prefetch_l2( const void* g ) { asm volatile(
 // rate-table entry at a 32-bit shared-memory address: the table base rides in the IDP.4A accumulator and the slot offset becomes the LDS immediate
 __device__ __forceinline__ uint32_t pyr_lds( uint32_t addr ) { uint32_t v; asm volatile( "ld.shared.u32 %0, [%1];" : "=r"( v ) : "r"( addr ) ); return v; }
 
+// max(w - o, 0) per 16-bit half.  Pels up to 1023 are fp16 subnormals (or zero) as they stand, and fp16 arithmetic keeps subnormals, so the difference of
+// two of them and its clamp are exact: the result's bits are the integer max(w - o, 0).
+__device__ __forceinline__ uint32_t pyr_relu_diff( uint32_t o, uint32_t w )
+{
+  uint32_t d;
+  asm( "fma.rn.relu.f16x2 %0, %1, %2, %3;" : "=r"( d ) : "r"( o ), "r"( 0xbc00bc00u ), "r"( w ) );
+  return d;
+}
+
+// box sums of two candidates (uint16 lanes of v) times the signed bytes of w, plus c
+__device__ __forceinline__ int pyr_dp2a_us( uint32_t v, uint32_t w, int c ) { int d; asm( "dp2a.lo.u32.s32 %0, %1, %2, %3;" : "=r"( d ) : "r"( v ), "r"( w ), "r"( c ) ); return d; }
+
 // one candidate row of one member: box sum + MV rate -> 8 packed (cost * 8 + slot) keys, running minimum; the SAD goes into the parent's sum.
-// mvRow = shared address of the rate tables + 4 * row bits
+// acc[k] = sum a + 2 sum max(b - a, 0); mvRow = shared address of the rate tables + 4 * row bits
 __device__ __forceinline__ uint32_t pyr_finish_row( const int (&acc)[8], const uint16_t* __restrict__ vrow, uint2 bw, uint32_t mvRow, uint32_t one, uint32_t eight,
                                                     uint32_t (&ps)[8] )
 {
@@ -132,7 +145,7 @@ __device__ __forceinline__ uint32_t pyr_finish_row( const int (&acc)[8], const u
   {
     const uint32_t a    = __dp4a( k < 4 ? bw.x : bw.y, 4u << ( 8 * ( k & 3 ) ), mvRow );                  // + 4 * column bits
     const uint32_t mvk  = pyr_lds( a + k * ( PYR_MVN * 4 ) );                                             // rate * 8 + k
-    const uint32_t sad  = __dp2a_lo( v[k >> 1], ( k & 1 ) ? 0x0100u : 0x0001u, (uint32_t) acc[k] );      // box sum + (sum a - 2 sum min)
+    const uint32_t sad  = (uint32_t) pyr_dp2a_us( v[k >> 1], ( k & 1 ) ? 0xff00u : 0x00ffu, acc[k] );  // - box sum: sum |a - b| = sum a - sum b + 2 sum max(b - a, 0)
     ps[k] = sad * one + ps[k];                                                                             // IMAD: keeps the add off the alu pipe
     const uint32_t key = sad * eight + mvk;
     bk = min( bk, key );
@@ -451,9 +464,11 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
           {
             const int b0 = 4 * q + m;
             const int sumA = sSumA[b0];
-            int accA[8], accB[8];
+            // per slot and row, max(b - a, 0) of the 32 pel-pair words (HFMA2.RELU, fma pipe) summed as two uint16 lanes: 32 * 1023 leaves no carry, and one
+            // IADD3 (alu pipe) adds two words
+            uint32_t pA[8], pB[8];
 #pragma unroll
-            for( int k = 0; k < 8; k++ ) { accA[k] = sumA; accB[k] = sumA; }
+            for( int k = 0; k < 8; k++ ) { pA[k] = 0u; pB[k] = 0u; }
             uint4 oPrev = make_uint4( 0, 0, 0, 0 );
 #pragma unroll
             for( int y = 0; y < 9; y++ )
@@ -470,8 +485,11 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
 #pragma unroll
                 for( int k = 0; k < 8; k++ )
 #pragma unroll
-                  for( int i = 0; i < 4; i++ )
-                    accA[k] = __dp2a_lo( (int) __vmins2( o[i], ( k & 1 ) ? d[i + ( k >> 1 )] : e[i + ( k >> 1 )] ), (int) 0x0000fefeu, accA[k] );
+                  for( int i = 0; i < 4; i += 2 )
+                  {
+                    const uint32_t wa = ( k & 1 ) ? d[i + ( k >> 1 )] : e[i + ( k >> 1 )], wb = ( k & 1 ) ? d[i + 1 + ( k >> 1 )] : e[i + 1 + ( k >> 1 )];
+                    pA[k] += pyr_relu_diff( o[i], wa ) + pyr_relu_diff( o[i + 1], wb );
+                  }
               }
               if( y > 0 )
               {
@@ -479,11 +497,17 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
 #pragma unroll
                 for( int k = 0; k < 8; k++ )
 #pragma unroll
-                  for( int i = 0; i < 4; i++ )
-                    accB[k] = __dp2a_lo( (int) __vmins2( o[i], ( k & 1 ) ? d[i + ( k >> 1 )] : e[i + ( k >> 1 )] ), (int) 0x0000fefeu, accB[k] );
+                  for( int i = 0; i < 4; i += 2 )
+                  {
+                    const uint32_t wa = ( k & 1 ) ? d[i + ( k >> 1 )] : e[i + ( k >> 1 )], wb = ( k & 1 ) ? d[i + 1 + ( k >> 1 )] : e[i + 1 + ( k >> 1 )];
+                    pB[k] += pyr_relu_diff( o[i], wa ) + pyr_relu_diff( o[i + 1], wb );
+                  }
               }
               oPrev = oCur;
             }
+            int accA[8], accB[8];
+#pragma unroll
+            for( int k = 0; k < 8; k++ ) { accA[k] = __dp2a_lo( (int) pA[k], 0x0202, sumA ); accB[k] = __dp2a_lo( (int) pB[k], 0x0202, sumA ); }
             // member epilogue
             const uint2 bw = *reinterpret_cast<const uint2*>( bb + cx0 );
             uint32_t bk = pyr_finish_row( accA, vrow, bw, mvBase + bb[nxp + cy], one, eight, psA );
