@@ -52,7 +52,8 @@ int         vvb_launch_count( const vvb_ctx* ctx, uint64_t* kernels_launched );
  * only ENQUEUE their copies and kernels on the context's stream and return; vvb_synchronize() is the completion point.  Host input buffers
  * stay borrowed and host output buffers undefined until then; use page-locked host memory, otherwise the copies degrade to blocking ones.
  * Work of one context stays ordered; independent contexts (one per worker, EncSlice.cpp:142-147) overlap each other's copies and kernels.
- * The *_block helpers that return a value always block. */
+ * The single-call helpers on borrowed host blocks (vvb_dist_block, vvb_sad_mask_block, vvb_sad_x5_block, vvb_fix_wsse_block, vvb_affine_sobel,
+ * vvb_affine_equal_coeff) always block: their results are in place when they return, in either mode. */
 int         vvb_set_async  ( vvb_ctx* ctx, int enable );   /* kernels this context has launched so far */
 
 /* measurement aid (bench.py): issue-rate probe of the packed-SAD instruction mix; no reference counterpart */

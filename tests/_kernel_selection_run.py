@@ -1,4 +1,4 @@
-"""Worker of test_kernel_selection in test_gpu_format_limits.py and test_gpu_mctf_limits.py: runs every case of the module's kernel_selection_cases() once
+"""Worker of test_kernel_selection in test_gpu_format_limits.py, test_gpu_mctf_limits.py, test_gpu_tu_limits.py and test_gpu_single_call.py: runs every case of the module's kernel_selection_cases() once
 under torch.profiler, in a process of its own, and prints one JSON line per case: {"case": label, "ok": the case's expectation holds, "kernels": names of the
 kernels in the trace}.
 usage: python tests/_kernel_selection_run.py [test module, default test_gpu_format_limits]"""

@@ -111,4 +111,5 @@ struct vvb_ctx
   //  - Work: the temporaries of a _dev call.  A _dev call that holds Work never calls another entry point that takes Work.
   void*          d_scratch[2] = {};
   size_t         d_scratchSize[2] = {};
+  std::vector<uint8_t> hostStage;      // host side of the single-call helpers' one upload (BlockCall in capi.cu)
 };
