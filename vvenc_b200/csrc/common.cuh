@@ -22,6 +22,9 @@ struct PlaneTable { Plane p[VVB_MAX_PLANES]; };
 
 __device__ __forceinline__ int ilog2_dev( int v ) { return 31 - __clz( v ); }
 
+// i / d for d > 0 given as inv = 1.0f / d: a float multiply instead of an integer division; exact for i < 2^20 and small divisors
+__device__ __forceinline__ int div_rcp( int i, float inv ) { return __float2int_rz( ( (float) i + 0.5f ) * inv ); }
+
 // ---- packed 16x2 arithmetic (SASS: VIMNMX.S16x2, IDP.2A) -------------------------------------------------------
 // sum over both signed 16-bit halves of |a - b|, added to acc:  |a-b| = max(a,b) - min(a,b)
 __device__ __forceinline__ int sad2_acc( uint32_t a, uint32_t b, int acc )

@@ -6,6 +6,7 @@
 //         (sobel_kernel, equal_coeff_kernel) and one block per CTA over a list of blocks (affine_eq_batch_kernel, SURVEY row a16).
 #pragma once
 #include "common.cuh"
+#include "packed_filter.cuh"
 
 namespace vvb {
 
@@ -44,7 +45,18 @@ __host__ __device__ inline MctfSmem mctf_smem( int maxDim ) { return mctf_smem( 
 
 __device__ __forceinline__ int32_t mctf_sat32( unsigned long long e ) { return (int32_t)( e < 0x7fffffffull ? e : 0x7fffffffull ); }
 
-__device__ __forceinline__ int mctf_div( int i, float inv ) { return __float2int_rz( ( (float) i + 0.5f ) * inv ); }   // exact for i < 2^20, divisors <= 64
+// the taps of 1/16-pel phase `phase` as a 6-tap filter over pels x-2 .. x+3, packed: the 8-tap set without its zero ends, or the 4-tap set
+// embedded as (0, t0, t1, t2, t3, 0)
+__device__ __forceinline__ PackedTaps<6> mctf_taps6( int tap4, int phase )
+{
+  int f[6];
+#pragma unroll
+  for( int t = 0; t < 6; t++ ) f[t] = tap4 ? ( t >= 1 && t <= 4 ? c_mctfF4[phase][t - 1] : 0 ) : c_mctfF8[phase][t + 1];
+  return pack_taps<6>( f );
+}
+
+// a filter pass's rounding with the clip to the pel range (motionErrorLumaFrac6/4 after both passes, applyFrac after the second)
+__device__ __forceinline__ int mctf_round_clip( int v, int maxv ) { return max( min( ( v + 32 ) >> 6, maxv ), 0 ); }
 
 // motionErrorLuma of one candidate by one warp (no early exit, unsaturated); region / t2: the warp's slices of shared memory (mctf_smem); every lane returns the error
 __device__ __forceinline__ unsigned mctf_warp_error( const Plane& orgPlane, const Plane& refPlane, const vvb_mctf_cand& c, int tap4, const MctfSmem& L, uint32_t* region, uint32_t* t2, int lane )
@@ -64,7 +76,7 @@ __device__ __forceinline__ unsigned mctf_warp_error( const Plane& orgPlane, cons
     const int16_t* buf = refPlane.origin + (ptrdiff_t)( c.y + dy ) * refPlane.stride + c.x + dx;
     for( int i = lane; i < w * h; i += 32 )
     {
-      const int y = mctf_div( i, invW ), x = i - y * w;
+      const int y = div_rcp( i, invW ), x = i - y * w;
       const int d = (int) __ldg( org + (ptrdiff_t) y * orgPlane.stride + x ) - (int) __ldg( buf + (ptrdiff_t) y * refPlane.stride + x );
       err += d * d;
     }
@@ -72,69 +84,37 @@ __device__ __forceinline__ unsigned mctf_warp_error( const Plane& orgPlane, cons
   else
   {
     dx >>= 4; dy >>= 4;                                  // MCTF.cpp:1136-1137 / :1151-1152 (arithmetic shift)
-    // taps as 6-tap filters f[0..5] over pels x-2 .. x+3 (rows y-2 .. y+3)
-    int fxv[6], fyv[6];
-#pragma unroll
-    for( int t = 0; t < 6; t++ )
-    {
-      fxv[t] = tap4 ? ( t >= 1 && t <= 4 ? c_mctfF4[fx][t - 1] : 0 ) : c_mctfF8[fx][t + 1];
-      fyv[t] = tap4 ? ( t >= 1 && t <= 4 ? c_mctfF4[fy][t - 1] : 0 ) : c_mctfF8[fy][t + 1];
-    }
-#define VVB_B4( a, b, c_, d ) ( (uint32_t)( (a) & 255 ) | ( (uint32_t)( (b) & 255 ) << 8 ) | ( (uint32_t)( (c_) & 255 ) << 16 ) | ( (uint32_t)( (d) & 255 ) << 24 ) )
-    const int xFA = (int) VVB_B4( fxv[0], fxv[1], fxv[2], fxv[3] ), xFB = (int) VVB_B4( fxv[4], fxv[5], 0, 0 );
-    const int xGA = (int) VVB_B4( 0, fxv[0], fxv[1], fxv[2] ),      xGB = (int) VVB_B4( fxv[3], fxv[4], fxv[5], 0 );
-    const int yFA = (int) VVB_B4( fyv[0], fyv[1], fyv[2], fyv[3] ), yFB = (int) VVB_B4( fyv[4], fyv[5], 0, 0 );
-    const int yGA = (int) VVB_B4( 0, fyv[0], fyv[1], fyv[2] ),      yGB = (int) VVB_B4( fyv[3], fyv[4], fyv[5], 0 );
-#undef VVB_B4
-#define VVB_E( a, b, c_, FA, FB ) __dp2a_lo( (int)(c_), FB, __dp2a_hi( (int)(b), FA, __dp2a_lo( (int)(a), FA, 0 ) ) )
-#define VVB_O( a, b, c_, d, GA, GB ) __dp2a_hi( (int)(d), GB, __dp2a_lo( (int)(c_), GB, __dp2a_hi( (int)(b), GA, __dp2a_lo( (int)(a), GA, 0 ) ) ) )
-#define VVB_RC( v ) max( min( ( (v) + 32 ) >> 6, maxv ), 0 )
+    const PackedTaps<6> X = mctf_taps6( tap4, fx ), Y = mctf_taps6( tap4, fy );
     // ---- stage the source region: rows y-2 .. y+h+3 (the last one only pairs up the row count), pels from the even pel at or below x-2
-    const int16_t* src0 = refPlane.origin + (ptrdiff_t)( c.y + dy - 2 ) * refPlane.stride + c.x + dx - 2;
-    const int o = (int)( ( reinterpret_cast<uintptr_t>( src0 ) >> 1 ) & 1 );            // plane rows are 16-byte aligned: same parity on every row
-    const uint32_t* srcW = reinterpret_cast<const uint32_t*>( src0 - o );
-    const int nW = ( w + 5 + o + 1 ) >> 1, rowsP = ( h + 6 ) & ~1;                      // words per row, rows rounded up to pairs
-    const float invNw = 1.0f / (float) nW;
-    const int strideW = refPlane.stride >> 1;
+    const int rowsP = ( h + 6 ) & ~1;
     __syncwarp();
-    for( int i = lane; i < rowsP * nW; i += 32 )
-    {
-      const int r = mctf_div( i, invNw ), k = i - r * nW;
-      region[r * PW + k] = __ldg( srcW + (ptrdiff_t) r * strideW + k );
-    }
+    const int o = stage_pel_pairs( region, PW, refPlane.origin + (ptrdiff_t)( c.y + dy - 2 ) * refPlane.stride + c.x + dx - 2, refPlane.stride, w + 5, rowsP, lane, 32 );
     __syncwarp();
     // ---- horizontal pass: item = (row pair rp, column pair cp) -> t2[rp][x], t2[rp][x+1] = packed ( row 2rp, row 2rp+1 )
     const int nRp = rowsP >> 1;
     for( int i = lane; i < nRp * hw; i += 32 )
     {
-      const int rp = mctf_div( i, invHw ), cp = i - rp * hw;
+      const int rp = div_rcp( i, invHw ), cp = i - rp * hw;
       const uint32_t* ra = region + ( 2 * rp ) * PW + cp;
-      const uint32_t* rb = ra + PW;
-      const uint32_t a0 = ra[0], a1 = ra[1], a2 = ra[2], a3 = ra[3], b0 = rb[0], b1 = rb[1], b2 = rb[2], b3 = rb[3];
-      int ha0, ha1, hb0, hb1;
-      if( o == 0 ) { ha0 = VVB_E( a0, a1, a2, xFA, xFB ); ha1 = VVB_O( a0, a1, a2, a3, xGA, xGB ); hb0 = VVB_E( b0, b1, b2, xFA, xFB ); hb1 = VVB_O( b0, b1, b2, b3, xGA, xGB ); }
-      else         { ha0 = VVB_O( a0, a1, a2, a3, xGA, xGB ); ha1 = VVB_E( a1, a2, a3, xFA, xFB ); hb0 = VVB_O( b0, b1, b2, b3, xGA, xGB ); hb1 = VVB_E( b1, b2, b3, xFA, xFB ); }
-      ha0 = VVB_RC( ha0 ); ha1 = VVB_RC( ha1 ); hb0 = VVB_RC( hb0 ); hb1 = VVB_RC( hb1 );
+      int2 ha, hb;
+      filter_row_pair<6>( ra, ra + PW, o, X, ha, hb );
       uint2 pk;
-      pk.x = (uint32_t) ha0 | ( (uint32_t) hb0 << 16 );
-      pk.y = (uint32_t) ha1 | ( (uint32_t) hb1 << 16 );
+      pk.x = (uint32_t) mctf_round_clip( ha.x, maxv ) | ( (uint32_t) mctf_round_clip( hb.x, maxv ) << 16 );
+      pk.y = (uint32_t) mctf_round_clip( ha.y, maxv ) | ( (uint32_t) mctf_round_clip( hb.y, maxv ) << 16 );
       *reinterpret_cast<uint2*>( t2 + rp * w + 2 * cp ) = pk;
     }
     __syncwarp();
     // ---- vertical pass + SSE: item = (output row pair yp, column x): rows 2yp (E on pairs yp..yp+2) and 2yp+1 (O on pairs yp..yp+3)
     for( int i = lane; i < ( h >> 1 ) * w; i += 32 )
     {
-      const int yp = mctf_div( i, invW ), x = i - yp * w;
+      const int yp = div_rcp( i, invW ), x = i - yp * w;
       const uint32_t* tp = t2 + yp * w + x;
-      const uint32_t p0 = tp[0], p1 = tp[w], p2 = tp[2 * w], p3 = tp[3 * w];
-      const int v0 = VVB_RC( VVB_E( p0, p1, p2, yFA, yFB ) ), v1 = VVB_RC( VVB_O( p0, p1, p2, p3, yGA, yGB ) );
+      const uint32_t p[4] = { tp[0], tp[w], tp[2 * w], tp[3 * w] };
+      const int2 v = filter_pair<6>( p, false, Y );
       const int16_t* op = org + (ptrdiff_t)( 2 * yp ) * orgPlane.stride + x;
-      const int d0 = v0 - (int) __ldg( op ), d1 = v1 - (int) __ldg( op + orgPlane.stride );
+      const int d0 = mctf_round_clip( v.x, maxv ) - (int) __ldg( op ), d1 = mctf_round_clip( v.y, maxv ) - (int) __ldg( op + orgPlane.stride );
       err += d0 * d0 + d1 * d1;
     }
-#undef VVB_E
-#undef VVB_O
-#undef VVB_RC
   }
   return __reduce_add_sync( 0xffffffffu, (unsigned) err );
 }
@@ -179,7 +159,7 @@ __host__ __device__ inline MctfGridSmem mctf_grid_smem( int maxDim, int step, in
   m.orgWords = ( maxDim >> 1 ) * maxDim;
   m.errWords = ( K1 * K1 + 1 ) & ~1;
   m.tapWords = 8 * K1;                                           // packed taps per grid column (x) and row (y)
-  m.tapOff   = ( m.winWords + m.hWords + m.orgWords + m.errWords + 3 ) & ~3;   // int4 entries: 16-byte aligned
+  m.tapOff   = ( m.winWords + m.hWords + m.orgWords + m.errWords + 3 ) & ~3;   // PackedTaps<6> entries: 16-byte aligned
   m.total    = m.tapOff + m.tapWords;
   return m;
 }
@@ -194,7 +174,7 @@ __global__ void __launch_bounds__( 256 ) mctf_grid_kernel( const __grid_constant
   uint32_t* hbuf = win + L.winWords;
   uint32_t* orgP = hbuf + L.hWords;
   unsigned* sErr = orgP + L.orgWords;                                       // exact up to 64 x 64 pels at 10 bits (4096 * 1023^2 < 2^32)
-  int4*     sTap = reinterpret_cast<int4*>( sGrid + L.tapOff );           // [2 * K1]: x columns, then y rows
+  PackedTaps<6>* sTap = reinterpret_cast<PackedTaps<6>*>( sGrid + L.tapOff );   // [2 * K1]: x columns, then y rows
   const int tid = threadIdx.x, T = blockDim.x;
   const int K1 = 2 * radius + 1, K = K1 * K1;
   const int maxv = ( 1 << refPlane.bitDepth ) - 1;
@@ -211,41 +191,25 @@ __global__ void __launch_bounds__( 256 ) mctf_grid_kernel( const __grid_constant
     const int dxMax = ( blk.mvx + radius * step ) >> 4, dyMax = ( blk.mvy + radius * step ) >> 4;
     const int rowsP = ( h + 6 + ( dyMax - dyMin ) + 1 ) & ~1;
     // ---- stage the window (rows y+dyMin-2 .., pels from the even pel at or below x+dxMin-2), the original block as row pairs, clear the errors
-    const int16_t* src0 = refPlane.origin + (ptrdiff_t)( blk.y + dyMin - 2 ) * refPlane.stride + blk.x + dxMin - 2;
-    const int o = (int)( ( reinterpret_cast<uintptr_t>( src0 ) >> 1 ) & 1 );
-    const uint32_t* srcW = reinterpret_cast<const uint32_t*>( src0 - o );
-    const int nW = ( w + 5 + ( dxMax - dxMin ) + o + 1 ) >> 1;
-    const float invNw = 1.0f / (float) nW;
-    const int strideW = refPlane.stride >> 1;
     __syncthreads();
-    for( int i = tid; i < rowsP * nW; i += T )
-    {
-      const int r = mctf_div( i, invNw ), k = i - r * nW;
-      win[r * PW + k] = __ldg( srcW + (ptrdiff_t) r * strideW + k );
-    }
+    const int o = stage_pel_pairs( win, PW, refPlane.origin + (ptrdiff_t)( blk.y + dyMin - 2 ) * refPlane.stride + blk.x + dxMin - 2, refPlane.stride,
+                                   w + 5 + ( dxMax - dxMin ), rowsP, tid, T );
     {
       const int16_t* org = orgPlane.origin + (ptrdiff_t) blk.y * orgPlane.stride + blk.x;
       for( int i = tid; i < hh * w; i += T )
       {
-        const int yp = mctf_div( i, invW ), x = i - yp * w;
+        const int yp = div_rcp( i, invW ), x = i - yp * w;
         const int16_t* op = org + (ptrdiff_t)( 2 * yp ) * orgPlane.stride + x;
         orgP[i] = (uint32_t)(uint16_t) __ldg( op ) | ( (uint32_t)(uint16_t) __ldg( op + orgPlane.stride ) << 16 );
       }
     }
     for( int k = tid; k < K; k += T ) sErr[k] = 0;
     __syncthreads();
-#define VVB_B4( a, b, c_, d ) ( (uint32_t)( (a) & 255 ) | ( (uint32_t)( (b) & 255 ) << 8 ) | ( (uint32_t)( (c_) & 255 ) << 16 ) | ( (uint32_t)( (d) & 255 ) << 24 ) )
-#define VVB_E( a, b, c_, FA, FB ) __dp2a_lo( (int)(c_), FB, __dp2a_hi( (int)(b), FA, __dp2a_lo( (int)(a), FA, 0 ) ) )
-#define VVB_O( a, b, c_, d, GA, GB ) __dp2a_hi( (int)(d), GB, __dp2a_lo( (int)(c_), GB, __dp2a_hi( (int)(b), GA, __dp2a_lo( (int)(a), GA, 0 ) ) ) )
-#define VVB_RC( v ) max( min( ( (v) + 32 ) >> 6, maxv ), 0 )
-#define VVB_TAPS( f, ph ) { _Pragma( "unroll" ) for( int t = 0; t < 6; t++ ) f[t] = tap4 ? ( t >= 1 && t <= 4 ? c_mctfF4[ph][t - 1] : 0 ) : c_mctfF8[ph][t + 1]; }
     // packed taps of every grid column / row (phase = vector & 15)
     for( int k = tid; k < 2 * K1; k += T )
     {
       const int mv = ( k < K1 ? blk.mvx : blk.mvy ) + ( ( k < K1 ? k : k - K1 ) - radius ) * step;
-      int f[6];
-      VVB_TAPS( f, mv & 15 )
-      sTap[k] = make_int4( (int) VVB_B4( f[0], f[1], f[2], f[3] ), (int) VVB_B4( f[4], f[5], 0, 0 ), (int) VVB_B4( 0, f[0], f[1], f[2] ), (int) VVB_B4( f[3], f[4], f[5], 0 ) );
+      sTap[k] = mctf_taps6( tap4, mv & 15 );
     }
     __syncthreads();
     const int perCol = ( rowsP >> 1 ) * hw;
@@ -256,22 +220,17 @@ __global__ void __launch_bounds__( 256 ) mctf_grid_kernel( const __grid_constant
       // ---- horizontal pass for gcount grid columns: item = (column, row pair, column pair)
       for( int it = tid; it < gcount * perCol; it += T )
       {
-        const int g = mctf_div( it, invPerCol ), rem = it - g * perCol;
-        const int rp = mctf_div( rem, invHw ), cp = rem - rp * hw;
+        const int g = div_rcp( it, invPerCol ), rem = it - g * perCol;
+        const int rp = div_rcp( rem, invHw ), cp = rem - rp * hw;
         const int mvx = blk.mvx + ( i0 + g - radius ) * step;
         const int e = ( mvx >> 4 ) - dxMin + o, eo = e & 1, ew = e >> 1;      // pel offset of this vector inside the window rows
-        const int4 tx = sTap[i0 + g];
-        const int xFA = tx.x, xFB = tx.y, xGA = tx.z, xGB = tx.w;
+        const PackedTaps<6> X = sTap[i0 + g];
         const uint32_t* ra = win + ( 2 * rp ) * PW + cp + ew;
-        const uint32_t* rb = ra + PW;
-        const uint32_t a0 = ra[0], a1 = ra[1], a2 = ra[2], a3 = ra[3], b0 = rb[0], b1 = rb[1], b2 = rb[2], b3 = rb[3];
-        int ha0, ha1, hb0, hb1;
-        if( eo == 0 ) { ha0 = VVB_E( a0, a1, a2, xFA, xFB ); ha1 = VVB_O( a0, a1, a2, a3, xGA, xGB ); hb0 = VVB_E( b0, b1, b2, xFA, xFB ); hb1 = VVB_O( b0, b1, b2, b3, xGA, xGB ); }
-        else          { ha0 = VVB_O( a0, a1, a2, a3, xGA, xGB ); ha1 = VVB_E( a1, a2, a3, xFA, xFB ); hb0 = VVB_O( b0, b1, b2, b3, xGA, xGB ); hb1 = VVB_E( b1, b2, b3, xFA, xFB ); }
-        ha0 = VVB_RC( ha0 ); ha1 = VVB_RC( ha1 ); hb0 = VVB_RC( hb0 ); hb1 = VVB_RC( hb1 );
+        int2 ha, hb;
+        filter_row_pair<6>( ra, ra + PW, eo, X, ha, hb );
         uint2 pk;
-        pk.x = (uint32_t) ha0 | ( (uint32_t) hb0 << 16 );
-        pk.y = (uint32_t) ha1 | ( (uint32_t) hb1 << 16 );
+        pk.x = (uint32_t) mctf_round_clip( ha.x, maxv ) | ( (uint32_t) mctf_round_clip( hb.x, maxv ) << 16 );
+        pk.y = (uint32_t) mctf_round_clip( ha.y, maxv ) | ( (uint32_t) mctf_round_clip( hb.y, maxv ) << 16 );
         *reinterpret_cast<uint2*>( hbuf + g * L.colWords + rp * w + 2 * cp ) = pk;
       }
       __syncthreads();
@@ -279,7 +238,7 @@ __global__ void __launch_bounds__( 256 ) mctf_grid_kernel( const __grid_constant
       if( hh * w <= T )                // one position per thread (blocks up to 16x16): decode it and fetch the original pels once
       {
         const bool act = tid < hh * w;
-        const int yp = mctf_div( tid, invW ), x = tid - yp * w;
+        const int yp = div_rcp( tid, invW ), x = tid - yp * w;
         const uint32_t ow = act ? orgP[tid] : 0u;
         const int o0 = (int)( ow & 0xffffu ), o1 = (int)( ow >> 16 );
         const uint32_t* hx = hbuf + x;
@@ -288,16 +247,14 @@ __global__ void __launch_bounds__( 256 ) mctf_grid_kernel( const __grid_constant
           for( int j = 0; j < K1; j++ )
           {
             const int q = ( ( blk.mvy + ( j - radius ) * step ) >> 4 ) - dyMin + 2 * yp;
-            const int4 ty = sTap[K1 + j];
+            const PackedTaps<6> Y = sTap[K1 + j];
             unsigned err = 0;
             if( act )
             {
               const uint32_t* tp = hx + ( q >> 1 ) * w;
-              const uint32_t p0 = tp[0], p1 = tp[w], p2 = tp[2 * w], p3 = tp[3 * w];
-              int v0, v1;
-              if( ( q & 1 ) == 0 ) { v0 = VVB_E( p0, p1, p2, ty.x, ty.y ); v1 = VVB_O( p0, p1, p2, p3, ty.z, ty.w ); }
-              else                 { v0 = VVB_O( p0, p1, p2, p3, ty.z, ty.w ); v1 = VVB_E( p1, p2, p3, ty.x, ty.y ); }
-              const int d0 = VVB_RC( v0 ) - o0, d1 = VVB_RC( v1 ) - o1;
+              const uint32_t p[4] = { tp[0], tp[w], tp[2 * w], tp[3 * w] };
+              const int2 v = filter_pair<6>( p, q & 1, Y );
+              const int d0 = mctf_round_clip( v.x, maxv ) - o0, d1 = mctf_round_clip( v.y, maxv ) - o1;
               err = d0 * d0 + d1 * d1;
             }
             err = __reduce_add_sync( 0xffffffffu, err );
@@ -313,20 +270,17 @@ __global__ void __launch_bounds__( 256 ) mctf_grid_kernel( const __grid_constant
         {
           const int mvy = blk.mvy + ( j - radius ) * step;
           const int q0 = ( mvy >> 4 ) - dyMin;                                 // first filtered row of output row 0
-          const int4 ty = sTap[K1 + j];
-          const int yFA = ty.x, yFB = ty.y, yGA = ty.z, yGB = ty.w;
+          const PackedTaps<6> Y = sTap[K1 + j];
           unsigned err = 0;
           for( int p = tid; p < hh * w; p += T )
           {
-            const int yp = mctf_div( p, invW ), x = p - yp * w;
+            const int yp = div_rcp( p, invW ), x = p - yp * w;
             const int q = q0 + 2 * yp;
             const uint32_t* tp = H + ( q >> 1 ) * w + x;
-            const uint32_t p0 = tp[0], p1 = tp[w], p2 = tp[2 * w], p3 = tp[3 * w];
-            int v0, v1;
-            if( ( q & 1 ) == 0 ) { v0 = VVB_E( p0, p1, p2, yFA, yFB ); v1 = VVB_O( p0, p1, p2, p3, yGA, yGB ); }
-            else                 { v0 = VVB_O( p0, p1, p2, p3, yGA, yGB ); v1 = VVB_E( p1, p2, p3, yFA, yFB ); }
+            const uint32_t pw[4] = { tp[0], tp[w], tp[2 * w], tp[3 * w] };
+            const int2 v = filter_pair<6>( pw, q & 1, Y );
             const uint32_t ow = orgP[p];
-            const int d0 = VVB_RC( v0 ) - (int)( ow & 0xffffu ), d1 = VVB_RC( v1 ) - (int)( ow >> 16 );
+            const int d0 = mctf_round_clip( v.x, maxv ) - (int)( ow & 0xffffu ), d1 = mctf_round_clip( v.y, maxv ) - (int)( ow >> 16 );
             err += d0 * d0 + d1 * d1;
           }
           err = __reduce_add_sync( 0xffffffffu, err );
@@ -335,11 +289,6 @@ __global__ void __launch_bounds__( 256 ) mctf_grid_kernel( const __grid_constant
       }
       __syncthreads();               // the filtered rows are consumed before the next group of columns overwrites them
     }
-#undef VVB_B4
-#undef VVB_E
-#undef VVB_O
-#undef VVB_RC
-#undef VVB_TAPS
     __syncthreads();
     for( int k = tid; k < K; k += T ) out[(size_t) b * K + k] = mctf_sat32( sErr[k] );
   }
@@ -407,65 +356,45 @@ __global__ void __launch_bounds__( 256 ) mctf_apply_kernel( const __grid_constan
     __syncthreads();
     for( int i = tid; i < h * w; i += T )
     {
-      const int y = mctf_div( i, invW ), x = i - y * w;
+      const int y = div_rcp( i, invW ), x = i - y * w;
       orgB[i] = __ldg( orgPlane.origin + (ptrdiff_t)( by + y ) * orgPlane.stride + bx + x );
     }
-#define VVB_B4( a, b_, c_, d ) ( (uint32_t)( (a) & 255 ) | ( (uint32_t)( (b_) & 255 ) << 8 ) | ( (uint32_t)( (c_) & 255 ) << 16 ) | ( (uint32_t)( (d) & 255 ) << 24 ) )
-#define VVB_E( a, b_, c_, FA, FB ) __dp2a_lo( (int)(c_), FB, __dp2a_hi( (int)(b_), FA, __dp2a_lo( (int)(a), FA, 0 ) ) )
-#define VVB_O( a, b_, c_, d, GA, GB ) __dp2a_hi( (int)(d), GB, __dp2a_lo( (int)(c_), GB, __dp2a_hi( (int)(b_), GA, __dp2a_lo( (int)(a), GA, 0 ) ) ) )
-#define VVB_R( v ) ( ( (v) + 32 ) >> 6 )
-#define VVB_TAPS( f, ph ) { _Pragma( "unroll" ) for( int t = 0; t < 6; t++ ) f[t] = tap4 ? ( t >= 1 && t <= 4 ? c_mctfF4[ph][t - 1] : 0 ) : c_mctfF8[ph][t + 1]; }
     for( int r = 0; r < par.numRefs; r++ )
     {
       const Plane refPlane = planes.p[par.refPlane[r]];
       const int4 mv = __ldg( mvs + (size_t) r * nBlocks + b );                        // x, y, error, rmsme
       int16_t* cr = corr + r * h * w;
       // ---- window: rows by+yInt-2 .., pels from the even pel at or below bx+xInt-2
-      const int16_t* src0 = refPlane.origin + (ptrdiff_t)( by + ( mv.y >> 4 ) - 2 ) * refPlane.stride + bx + ( mv.x >> 4 ) - 2;
-      const int o = (int)( ( reinterpret_cast<uintptr_t>( src0 ) >> 1 ) & 1 );
-      const uint32_t* srcW = reinterpret_cast<const uint32_t*>( src0 - o );
-      const int nW = ( w + 5 + o + 1 ) >> 1, rowsP = ( h + 6 ) & ~1;
-      const float invNw = 1.0f / (float) nW;
-      const int strideW = refPlane.stride >> 1;
+      const int rowsP = ( h + 6 ) & ~1;
       __syncthreads();                                   // previous reference's readers of win / hbuf are done
-      for( int i = tid; i < rowsP * nW; i += T )
-      {
-        const int rr = mctf_div( i, invNw ), k = i - rr * nW;
-        win[rr * PW + k] = __ldg( srcW + (ptrdiff_t) rr * strideW + k );
-      }
+      const int o = stage_pel_pairs( win, PW, refPlane.origin + (ptrdiff_t)( by + ( mv.y >> 4 ) - 2 ) * refPlane.stride + bx + ( mv.x >> 4 ) - 2, refPlane.stride,
+                                     w + 5, rowsP, tid, T );
       if( tid < 3 ) sI[tid] = 0;
       if( tid < 2 ) sAcc[tid] = 0ull;
       __syncthreads();
-      int f[6];
-      VVB_TAPS( f, mv.x & 15 )
-      const int xFA = (int) VVB_B4( f[0], f[1], f[2], f[3] ), xFB = (int) VVB_B4( f[4], f[5], 0, 0 );
-      const int xGA = (int) VVB_B4( 0, f[0], f[1], f[2] ),    xGB = (int) VVB_B4( f[3], f[4], f[5], 0 );
+      const PackedTaps<6> X = mctf_taps6( tap4, mv.x & 15 );
       for( int it = tid; it < ( rowsP >> 1 ) * hw; it += T )
       {
-        const int rp = mctf_div( it, invHw ), cp = it - rp * hw;
+        const int rp = div_rcp( it, invHw ), cp = it - rp * hw;
         const uint32_t* ra = win + ( 2 * rp ) * PW + cp;
-        const uint32_t* rb = ra + PW;
-        const uint32_t a0 = ra[0], a1 = ra[1], a2 = ra[2], a3 = ra[3], b0 = rb[0], b1 = rb[1], b2 = rb[2], b3 = rb[3];
-        int ha0, ha1, hb0, hb1;
-        if( o == 0 ) { ha0 = VVB_E( a0, a1, a2, xFA, xFB ); ha1 = VVB_O( a0, a1, a2, a3, xGA, xGB ); hb0 = VVB_E( b0, b1, b2, xFA, xFB ); hb1 = VVB_O( b0, b1, b2, b3, xGA, xGB ); }
-        else         { ha0 = VVB_O( a0, a1, a2, a3, xGA, xGB ); ha1 = VVB_E( a1, a2, a3, xFA, xFB ); hb0 = VVB_O( b0, b1, b2, b3, xGA, xGB ); hb1 = VVB_E( b1, b2, b3, xFA, xFB ); }
+        int2 ha, hb;
+        filter_row_pair<6>( ra, ra + PW, o, X, ha, hb );
         uint2 pk;                                        // first pass is NOT clipped (MCTF.cpp:284): signed 16-bit halves
-        pk.x = ( (uint32_t) VVB_R( ha0 ) & 0xffffu ) | ( (uint32_t) VVB_R( hb0 ) << 16 );
-        pk.y = ( (uint32_t) VVB_R( ha1 ) & 0xffffu ) | ( (uint32_t) VVB_R( hb1 ) << 16 );
+        pk.x = ( (uint32_t)( ( ha.x + 32 ) >> 6 ) & 0xffffu ) | ( (uint32_t)( ( hb.x + 32 ) >> 6 ) << 16 );
+        pk.y = ( (uint32_t)( ( ha.y + 32 ) >> 6 ) & 0xffffu ) | ( (uint32_t)( ( hb.y + 32 ) >> 6 ) << 16 );
         *reinterpret_cast<uint2*>( hbuf + rp * w + 2 * cp ) = pk;
       }
       __syncthreads();
-      VVB_TAPS( f, mv.y & 15 )
-      const int yFA = (int) VVB_B4( f[0], f[1], f[2], f[3] ), yFB = (int) VVB_B4( f[4], f[5], 0, 0 );
-      const int yGA = (int) VVB_B4( 0, f[0], f[1], f[2] ),    yGB = (int) VVB_B4( f[3], f[4], f[5], 0 );
+      const PackedTaps<6> Y = mctf_taps6( tap4, mv.y & 15 );
       const bool doPlanar = ( mv.w & 0xffff ) > 0 && par.planar && w == h && w <= 32;
       int s1 = 0, s2 = 0, s0 = 0;
       for( int p = tid; p < hh * w; p += T )
       {
-        const int yp = mctf_div( p, invW ), x = p - yp * w;
+        const int yp = div_rcp( p, invW ), x = p - yp * w;
         const uint32_t* tp = hbuf + yp * w + x;
-        const uint32_t p0 = tp[0], p1 = tp[w], p2 = tp[2 * w], p3 = tp[3 * w];
-        const int v0 = max( min( VVB_R( VVB_E( p0, p1, p2, yFA, yFB ) ), maxv ), 0 ), v1 = max( min( VVB_R( VVB_O( p0, p1, p2, p3, yGA, yGB ) ), maxv ), 0 );
+        const uint32_t pw[4] = { tp[0], tp[w], tp[2 * w], tp[3 * w] };
+        const int2 v = filter_pair<6>( pw, false, Y );
+        const int v0 = mctf_round_clip( v.x, maxv ), v1 = mctf_round_clip( v.y, maxv );
         cr[( 2 * yp ) * w + x] = (int16_t) v0; cr[( 2 * yp + 1 ) * w + x] = (int16_t) v1;
         if( doPlanar )
         {
@@ -498,7 +427,7 @@ __global__ void __launch_bounds__( 256 ) mctf_apply_kernel( const __grid_constan
         if( b0 | b1 | b2 )
           for( int i = tid; i < h * w; i += T )
           {
-            const int y = mctf_div( i, invW ), x = i - y * w;
+            const int y = div_rcp( i, invW ), x = i - y * w;
             const int pc = ( b0 + b1 * x + b2 * y + 256 ) >> 9;
             cr[i] = (int16_t) max( 0, min( maxv, (int) cr[i] - pc ) );
           }
@@ -509,7 +438,7 @@ __global__ void __launch_bounds__( 256 ) mctf_apply_kernel( const __grid_constan
         unsigned long long var = 0, dsum = 0;
         for( int i = tid; i < h * w; i += T )
         {
-          const int y = mctf_div( i, invW ), x = i - y * w;
+          const int y = div_rcp( i, invW ), x = i - y * w;
           const int diff = (int) orgB[i] - (int) cr[i];
           var += (unsigned)( diff * diff );
           if( x != w - 1 ) { const int dR = (int) orgB[i + 1] - (int) cr[i + 1]; dsum += (unsigned)( ( dR - diff ) * ( dR - diff ) ); }
@@ -552,7 +481,7 @@ __global__ void __launch_bounds__( 256 ) mctf_apply_kernel( const __grid_constan
     // ---- per-pel blend (MCTF.cpp:491-517)
     for( int i = tid; i < h * w; i += T )
     {
-      const int y = mctf_div( i, invW ), x = i - y * w;
+      const int y = div_rcp( i, invW ), x = i - y * w;
       const int orgVal = orgB[i];
       float temporalWeightSum = 1.0f;
       float newVal = (float) orgVal;
@@ -570,11 +499,6 @@ __global__ void __launch_bounds__( 256 ) mctf_apply_kernel( const __grid_constan
       sampleVal = max( 0, min( maxv, sampleVal ) );
       out[(size_t)( by + y ) * par.outStride + bx + x] = (int16_t) sampleVal;
     }
-#undef VVB_B4
-#undef VVB_E
-#undef VVB_O
-#undef VVB_R
-#undef VVB_TAPS
   }
 }
 
@@ -589,14 +513,14 @@ __global__ void mctf_calc_var_kernel( const __grid_constant__ Plane plane, const
   const int16_t* org = plane.origin + (ptrdiff_t) c.y * plane.stride + c.x;
   const float invW = 1.0f / (float) w;
   int avg = 0;
-  for( int i = lane; i < w * h; i += 32 ) { const int y = mctf_div( i, invW ), x = i - y * w; avg += __ldg( org + (ptrdiff_t) y * plane.stride + x ); }
+  for( int i = lane; i < w * h; i += 32 ) { const int y = div_rcp( i, invW ), x = i - y * w; avg += __ldg( org + (ptrdiff_t) y * plane.stride + x ); }
   avg = __reduce_add_sync( 0xffffffffu, avg );
   avg <<= 4;
   avg = avg / ( w * h );
   long long var = 0;
   for( int i = lane; i < w * h; i += 32 )
   {
-    const int y = mctf_div( i, invW ), x = i - y * w;
+    const int y = div_rcp( i, invW ), x = i - y * w;
     const int pix = (int) __ldg( org + (ptrdiff_t) y * plane.stride + x ) << 4;
     var += (long long)( ( pix - avg ) * ( pix - avg ) );
   }

@@ -267,7 +267,7 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
             v[u] = 0u;
             if( i < total )
             {
-              const int r = fast_div( i, inv ), c = i - r * wsw;
+              const int r = div_rcp( i, inv ), c = i - r * wsw;
               if( c < validWords ) v[u] = __ldg( reinterpret_cast<const uint32_t*>( src + (ptrdiff_t) r * refPlane.stride ) + c );
             }
           }
@@ -290,7 +290,7 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
             v[u] = 0;
             if( i < total )
             {
-              const int r = fast_div( i, inv ), c = i - r * ws;
+              const int r = div_rcp( i, inv ), c = i - r * ws;
               if( c < validW ) v[u] = __ldg( src + (ptrdiff_t) r * refPlane.stride + c );
             }
           }
@@ -329,7 +329,7 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
       const float inv = 1.0f / (float) cStrips;
       for( int t = tid; t < nTasks; t += nthr )
       {
-        const int r = fast_div( t, inv ), st = t - r * cStrips;
+        const int r = div_rcp( t, inv ), st = t - r * cStrips;
         const uint32_t* row = win0w + r * wsw + st * 4;
         const uint4 a = *reinterpret_cast<const uint4*>( row ), b = *reinterpret_cast<const uint4*>( row + 4 );
         const uint32_t w[8] = { a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w };
@@ -349,7 +349,7 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
       const float invB = 1.0f / (float) L.bStride;
       for( int t = tid; t < NBLK * L.bStride; t += nthr )
       {
-        const int bid = fast_div( t, invB ), e = t - bid * L.bStride;
+        const int bid = div_rcp( t, invB ), e = t - bid * L.bStride;
         const int2 pr = sPred[bid];
         unsigned char v;
         if( e < nxp ) v = e < nx ? (unsigned char) eg_bits( ( ( rb.left + e ) * ( 1 << par.costScale ) - pr.x ) >> par.imvShift ) : (unsigned char) PYR_PAD_BITS;
@@ -442,8 +442,8 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
         {
           const unsigned mask = maskS;
           int q, pr, st;
-          if( it < itemsMain ) { q = fast_div( it, invPerQm ); const int rem = it - q * perQm; pr = fast_div( rem, invMain ); st = rem - pr * nMain; }
-          else { const int i2 = it - itemsMain; q = fast_div( i2, invPerQt ); const int rem = i2 - q * perQt; const int ts = fast_div( rem, invPairs ); pr = rem - ts * nPairs; st = nMain + ts; }
+          if( it < itemsMain ) { q = div_rcp( it, invPerQm ); const int rem = it - q * perQm; pr = div_rcp( rem, invMain ); st = rem - pr * nMain; }
+          else { const int i2 = it - itemsMain; q = div_rcp( i2, invPerQt ); const int rem = i2 - q * perQt; const int ts = div_rcp( rem, invPairs ); pr = rem - ts * nPairs; st = nMain + ts; }
           const int cy = 2 * pr, cx0 = 8 * st;
           const bool validB = cy + 1 < ny;
           const int lead = __ffs( mask ) - 1;
@@ -559,8 +559,8 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
           // 15 window rows its 8 vectors touch: window row r meets original row r - c for vector c.
           const unsigned mask = maskC;
           const int ic = it - itemsStrip;
-          const int q = fast_div( ic, invPerQc ), rem = ic - q * perQc;
-          const int ci = fast_div( rem, invNv ), g = rem - ci * nV;
+          const int q = div_rcp( ic, invPerQc ), rem = ic - q * perQc;
+          const int ci = div_rcp( rem, invNv ), g = rem - ci * nV;
           const int cx = 8 * nFull + ci, cy0 = 8 * g;
           const int lead = __ffs( mask ) - 1;
           const bool uni = __all_sync( mask, q == __shfl_sync( mask, q, lead ) );
@@ -658,7 +658,7 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
       for( int j = 0; j < NTOP; j++ ) best[j] = ~0ull;
       for( int o = tid; o < nx * ny; o += nthr )
       {
-        const int cy = fast_div( o, invNx ), cx = o - cy * nx;
+        const int cy = div_rcp( o, invNx ), cx = o - cy * nx;
         const int ti = cy * nxp + ( cx & 7 ) * nStrips + ( cx >> 3 );
         uint32_t sum = 0u;
 #pragma unroll

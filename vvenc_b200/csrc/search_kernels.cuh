@@ -79,8 +79,6 @@ __host__ __device__ inline SearchSmem search_smem( int w, int h, int nx, int ny,
   return s;
 }
 
-__device__ __forceinline__ int fast_div( int i, float inv ) { return __float2int_rz( ( (float) i + 0.5f ) * inv ); }   // exact for i < 2^20, small divisors
-
 // TMA window staging: tmap describes the whole padded reference plane (uint16 elements), box = (ws x winH) of the launch's
 // largest window; (tmaNx, tmaNy, tmaQuad) say which window geometry the box was built for -- blocks with another geometry
 // use the load/store staging loop.  The copy is one cp.async.bulk.tensor.2d per CTA (any start alignment, zero fill outside).
@@ -268,7 +266,7 @@ __global__ void __launch_bounds__( PARENT ? 256 : 384, PARENT ? 3 : 2 ) sad_sear
             v[u] = 0u;
             if( i < total )
             {
-              const int r = fast_div( i, inv ), c = i - r * wpr;
+              const int r = div_rcp( i, inv ), c = i - r * wpr;
               if( c < validWords ) v[u] = __ldg( reinterpret_cast<const uint32_t*>( src + (ptrdiff_t) r * refPlane.stride ) + c );
             }
           }
@@ -290,7 +288,7 @@ __global__ void __launch_bounds__( PARENT ? 256 : 384, PARENT ? 3 : 2 ) sad_sear
             v[u] = 0;
             if( i < total )
             {
-              const int r = fast_div( i, inv ), c = i - r * ws;
+              const int r = div_rcp( i, inv ), c = i - r * ws;
               if( c < validW ) v[u] = __ldg( src + (ptrdiff_t) r * refPlane.stride + c );
             }
           }
@@ -335,7 +333,7 @@ __global__ void __launch_bounds__( PARENT ? 256 : 384, PARENT ? 3 : 2 ) sad_sear
       const float inv = 1.0f / (float) L.nStripsV;
       for( int t = tid; t < nTasks; t += nthr )
       {
-        const int r = fast_div( t, inv ), st = t - r * L.nStripsV;
+        const int r = div_rcp( t, inv ), st = t - r * L.nStripsV;
         const int16_t* row = win + r * ws + st * SS_STRIP;
         int s = 0;
         for( int x = 0; x < w; x++ ) s += row[x];
@@ -380,8 +378,8 @@ __global__ void __launch_bounds__( PARENT ? 256 : 384, PARENT ? 3 : 2 ) sad_sear
       unsigned long long bestKey = ~0ull; int curMem = -1;
       for( int it = tid; it < items; it += nthr )
       {
-        const int mem = fast_div( it, invPer ), loc = it - mem * perMem;
-        const int cy = fast_div( loc, invStr ), st = loc - cy * nStrips;
+        const int mem = div_rcp( it, invPer ), loc = it - mem * perMem;
+        const int cy = div_rcp( loc, invStr ), st = loc - cy * nStrips;
         const int bx = mem & ( nbx - 1 ), by = mem >> ( nbx - 1 );
         const int cx0 = st * SS_STRIP;
         if( mem != curMem )
@@ -438,7 +436,7 @@ __global__ void __launch_bounds__( PARENT ? 256 : 384, PARENT ? 3 : 2 ) sad_sear
       KT key4[4] = { KMAX, KMAX, KMAX, KMAX }, keyP = KMAX;
       for( int it = tid; it < perMem; it += nthr )
       {
-        const int cy = fast_div( it, invStr ), st = it - cy * nStrips;
+        const int cy = div_rcp( it, invStr ), st = it - cy * nStrips;
         const int cx0 = st * SS_STRIP;
         const int pByBits = pBitsY[cy];
         uint32_t psad[SS_STRIP];
@@ -582,7 +580,7 @@ __global__ void __launch_bounds__( 256 ) sad_table_sum_kernel( const vvb_block* 
   {
     const uint32_t s = __ldg( c0 + o ) + __ldg( c0 + childStride + o ) + __ldg( c0 + 2 * (size_t) childStride + o ) + __ldg( c0 + 3 * (size_t) childStride + o );
     if( outTables ) outTables[(size_t) blockIdx.x * outStride + o] = s;
-    const int cy = fast_div( o, inv ), cx = o - cy * nx;
+    const int cy = div_rcp( o, inv ), cx = o - cy * nx;
     const uint32_t bits = (uint32_t)( sBitsX[cx] + sBitsY[cy] );
     const unsigned long long key = ( ( (unsigned long long) s + sMv[bits < VVB_MVCOST_ENTRIES ? bits : VVB_MVCOST_ENTRIES - 1] ) << 16 ) | (unsigned) o;
     best = key < best ? key : best;
@@ -977,9 +975,9 @@ __global__ void __launch_bounds__( 256 ) had8_direct_kernel( const __grid_consta
     __syncthreads();
     for( int it = tid; it < nSlot * perSlot; it += nthr )
     {
-      const int j = fast_div( it, invPer ), loc = it - j * perSlot;
-      const int k = fast_div( loc, invT ), t = loc - k * T;
-      const int ty = fast_div( t, invTx ), tx = t - ty * tilesX;
+      const int j = div_rcp( it, invPer ), loc = it - j * perSlot;
+      const int k = div_rcp( loc, invT ), t = loc - k * T;
+      const int ty = div_rcp( t, invTx ), tx = t - ty * tilesX;
       const vvb_block blk = sBlk[j];
       const vvb_mv pm = sPat[k];
       const int mx = blk.start_x + pm.dx, my = blk.start_y + pm.dy;
