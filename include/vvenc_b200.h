@@ -375,6 +375,36 @@ int vvb_tu_roundtrip_dev( vvb_ctx* ctx, const vvb_tu_par* par, const int16_t* de
 int vvb_tu_roundtrip_planes_dev( vvb_ctx* ctx, const vvb_tu_par* par, int org_plane, int pred_plane, const vvb_block* dev_blocks, int n,
                           int16_t* dev_q, int16_t* dev_reco, vvb_tu_result* dev_res, uint8_t* dev_need_rdoq );
 
+/* The same TU candidate with the quantiser the slice runs for it, in one call: what DepQuant::quant / QuantRDOQ2::quant (DepQuant.cpp:1462-1490,
+ * QuantRDOQ2.cpp:247-301) do inside TrQuant::transformNxN, then the round trip above.  Per TU:
+ *   1. residual = org - pred; the forward transform (with LFNST when par->lfnst_idx is set) and need_rdoq (Quant::xNeedRDOQ) exactly as vvb_fwd_trquant;
+ *   2. the levels: zero (abs_sum 0, last_pos -1) where `selective` (picture->useSelectiveRdoq) is set and need_rdoq is 0, otherwise those of vvb_rdoq (quantiser 1,
+ *      QuantRDOQ2::xRateDistOptQuantFast, m_RDOQ == 2: presets faster and fast) or of vvb_dep_quant (quantiser 2, DepQuant::xQuantDQ: presets medium to slower) with
+ *      the same parameters and rates, on the context's current RDOQ / DepQuant engine;
+ *   3. abs_sum > 0: the dequantiser that belongs to the quantiser (Quant::dequant after fast RDOQ, DepQuant::dequant at QP + 1 after the trellis) and the inverse
+ *      transform as vvb_inv_trquant; otherwise the residual is zero;
+ *   4. reco = clip( pred + residual ) and dist_reco / dist_resi / dist_zero as vvb_tu_result defines them.  abs_sum and last_pos are the quantiser's.
+ * need_rdoq (nullable) is returned whether or not `selective` is set.  The chroma distortion weight of getDistPart stays with the caller.  Luma and chroma
+ * (par->is_chroma) TUs with sides 4..64 and every MTS pair the forward transform takes; bit depth 8 or 10.
+ * Errors: quantiser other than 1 or 2, par->dep_quant set for quantiser 1 or clear for quantiser 2 (the dequantiser would not match), sign_hiding with quantiser 2
+ * (a slice cannot signal both), null quantiser parameters or rates: VVB_ERR_ARG; the parameter errors of vvb_rdoq / vvb_dep_quant as those calls give them;
+ * transform_skip (skipped and BDPCM TUs go through vvb_rdoq_ts / vvb_rdoq_bdpcm) and bit depths other than 8 or 10: VVB_ERR_UNSUPPORTED.
+ * Engines: the forward and the inverse each follow the rule of vvb_set_tensor_transform over org, pred, q and reco (the quantiser's sign-bit hiding does not keep
+ * the forward off the tensor engine); the intermediates live in the context's work arena. */
+typedef struct
+{
+  int32_t quantiser;                                          /* 1 = fast RDOQ (as vvb_rdoq), 2 = dependent quantisation (as vvb_dep_quant)  */
+  int32_t selective;                                          /* picture->useSelectiveRdoq: TUs whose need_rdoq is 0 get no levels           */
+  const vvb_rdoq_par* rq; const vvb_rdoq_rates* rq_rates;     /* quantiser 1                                                                 */
+  const vvb_dq_par*   dq; const vvb_dq_rates*   dq_rates;     /* quantiser 2                                                                 */
+} vvb_tu_quant;
+int vvb_tu_roundtrip_rdo    ( vvb_ctx* ctx, const vvb_tu_par* par, const vvb_tu_quant* quant, const int16_t* org, const int16_t* pred, int n,
+                              int16_t* q, int16_t* reco, vvb_tu_result* res, uint8_t* need_rdoq );
+int vvb_tu_roundtrip_rdo_dev( vvb_ctx* ctx, const vvb_tu_par* par, const vvb_tu_quant* quant, const int16_t* dev_org, const int16_t* dev_pred, int n,
+                              int16_t* dev_q, int16_t* dev_reco, vvb_tu_result* dev_res, uint8_t* dev_need_rdoq );
+int vvb_tu_roundtrip_rdo_planes_dev( vvb_ctx* ctx, const vvb_tu_par* par, const vvb_tu_quant* quant, int org_plane, int pred_plane, const vvb_block* dev_blocks, int n,
+                              int16_t* dev_q, int16_t* dev_reco, vvb_tu_result* dev_res, uint8_t* dev_need_rdoq );
+
 /* ---- MCTF block matching (CommonLib/MCTF.cpp:122-257 via MCTF::motionErrorLuma :1099-1164) -----------------
  * Every MCTF entry (error batch, search grid, calc_var, estimate_level, estimate_pyramid, apply) takes planes of up to 10 bits and returns
  * VVB_ERR_UNSUPPORTED when the original or the reference is wider (MCTF.cpp:1313 CHECKD).  Errors are exact SSEs while they fit int32 and saturate to

@@ -63,6 +63,11 @@ class vvb_rdoq_par(ctypes.Structure):
     _fields_ = [('lam', ctypes.c_double), ('thr_val', ctypes.c_int32), ('sbt_zero_out', ctypes.c_int32), ('pad', ctypes.c_int32 * 2)]
 
 
+class vvb_tu_quant(ctypes.Structure):
+    _fields_ = [('quantiser', ctypes.c_int32), ('selective', ctypes.c_int32), ('rq', ctypes.POINTER(vvb_rdoq_par)), ('rq_rates', ctypes.POINTER(vvb_rdoq_rates)),
+                ('dq', ctypes.POINTER(vvb_dq_par)), ('dq_rates', ctypes.POINTER(vvb_dq_rates))]
+
+
 class vvb_level_io(ctypes.Structure):
     _fields_ = [('blocks', ctypes.c_void_p), ('count', ctypes.c_int32), ('best', ctypes.c_void_p), ('refine_cost', ctypes.c_void_p), ('q', ctypes.c_void_p),
                 ('abs_sum', ctypes.c_void_p), ('last_pos', ctypes.c_void_p), ('need_rdoq', ctypes.c_void_p), ('tu', vvb_tu_par), ('packed_q', ctypes.c_void_p), ('packed_offsets', ctypes.c_void_p)]
@@ -156,6 +161,9 @@ SYMBOLS = {
     'vvb_tu_roundtrip': (c_i, [c_p, ctypes.POINTER(vvb_tu_par), c_p, c_p, c_i, c_p, c_p, c_p, c_p]),
     'vvb_tu_roundtrip_dev': (c_i, [c_p, ctypes.POINTER(vvb_tu_par), c_p, c_p, c_i, c_p, c_p, c_p, c_p]),
     'vvb_tu_roundtrip_planes_dev': (c_i, [c_p, ctypes.POINTER(vvb_tu_par), c_i, c_i, c_p, c_i, c_p, c_p, c_p, c_p]),
+    'vvb_tu_roundtrip_rdo': (c_i, [c_p, ctypes.POINTER(vvb_tu_par), ctypes.POINTER(vvb_tu_quant), c_p, c_p, c_i, c_p, c_p, c_p, c_p]),
+    'vvb_tu_roundtrip_rdo_dev': (c_i, [c_p, ctypes.POINTER(vvb_tu_par), ctypes.POINTER(vvb_tu_quant), c_p, c_p, c_i, c_p, c_p, c_p, c_p]),
+    'vvb_tu_roundtrip_rdo_planes_dev': (c_i, [c_p, ctypes.POINTER(vvb_tu_par), ctypes.POINTER(vvb_tu_quant), c_i, c_i, c_p, c_i, c_p, c_p, c_p, c_p]),
     'vvb_mctf_error_batch': (c_i, [c_p, c_i, c_i, c_p, c_i, c_i, c_p]),
     'vvb_mctf_search_grid': (c_i, [c_p, c_i, c_i, c_p, c_i, c_i, c_i, c_i, c_p]),
     'vvb_mctf_search_grid_dev': (c_i, [c_p, c_i, c_i, c_p, c_i, c_i, c_i, c_i, c_p]),

@@ -374,6 +374,54 @@ class CostEngine:
         return dict(q=d_q.cpu().numpy().reshape(n, par.h, par.w), reco=d_reco.cpu().numpy().reshape(n, par.h, par.w) if want_reco else None,
                     res=np.frombuffer(d_res.cpu().numpy().tobytes(), dtype=L.TU_RESULT_DT).copy(), need_rdoq=d_nr.cpu().numpy())
 
+    def _tu_quant(self, quantiser, rates, lam, thr_val, sbt_zero_out, dq_thr_val, zero_out, scalar_members, selective):
+        """vvb_tu_quant of quantiser 1 (fast RDOQ: rates as rdoq_rates takes them) or 2 (dependent quantisation: rates as dq_rates takes them), and the
+        structures it points to (kept alive by the caller while the call runs)"""
+        tq = L.vvb_tu_quant(int(quantiser), int(selective))
+        keep = []
+        if quantiser == 1:
+            r = rates if isinstance(rates, L.vvb_rdoq_rates) else self.rdoq_rates(rates)
+            rq = L.vvb_rdoq_par(float(lam), int(thr_val), int(sbt_zero_out))
+            tq.rq = ctypes.pointer(rq); tq.rq_rates = ctypes.pointer(r); keep += [r, rq]
+        elif quantiser == 2:
+            r = rates if isinstance(rates, L.vvb_dq_rates) else self.dq_rates(rates)
+            dq = L.vvb_dq_par(float(lam), int(dq_thr_val), int(zero_out), int(scalar_members), 0)
+            tq.dq = ctypes.pointer(dq); tq.dq_rates = ctypes.pointer(r); keep += [r, dq]
+        return tq, keep
+
+    def tu_roundtrip_rdo(self, par, org, pred, quantiser, rates, lam, *, thr_val=8, sbt_zero_out=False, dq_thr_val=8, zero_out=False, scalar_members=False,
+                         selective=True, want_reco=True):
+        """org, pred: int16 [n][h][w] compact.  residual -> transform -> fast RDOQ (quantiser 1) or dependent quantisation (quantiser 2) -> the matching
+        dequantiser and inverse when abs_sum > 0 -> reconstruct -> SSE, in one call.  par.dep_quant must be set exactly for quantiser 2.
+        Returns dict(q, reco, res (TU_RESULT_DT), need_rdoq) as tu_roundtrip does."""
+        org = np.ascontiguousarray(org, dtype=np.int16); pred = np.ascontiguousarray(pred, dtype=np.int16)
+        n = org.shape[0]
+        tq, keep = self._tu_quant(quantiser, rates, lam, thr_val, sbt_zero_out, dq_thr_val, zero_out, scalar_members, selective)
+        q = np.zeros((n, par.h, par.w), dtype=np.int16)
+        reco = np.zeros((n, par.h, par.w), dtype=np.int16) if want_reco else None
+        res = np.zeros(n, dtype=L.TU_RESULT_DT); nr = np.zeros(n, dtype=np.uint8)
+        self._chk(self.lib.vvb_tu_roundtrip_rdo(self.h, ctypes.byref(par), ctypes.byref(tq), _p(org), _p(pred), n, _p(q), _p(reco), _p(res), _p(nr)))
+        return dict(q=q, reco=reco, res=res, need_rdoq=nr)
+
+    def tu_roundtrip_rdo_planes(self, par, org_plane, pred_plane, blocks, quantiser, rates, lam, *, thr_val=8, sbt_zero_out=False, dq_thr_val=8, zero_out=False,
+                                scalar_members=False, selective=True, want_reco=True):
+        """tu_roundtrip_rdo with org / pred taken from resident planes (blocks: BLOCK_DT, prediction displaced by start_x/start_y).
+        Device-resident entry point wrapped with torch buffers."""
+        import torch
+        blocks = np.ascontiguousarray(blocks, dtype=L.BLOCK_DT)
+        n = len(blocks); area = par.w * par.h
+        tq, keep = self._tu_quant(quantiser, rates, lam, thr_val, sbt_zero_out, dq_thr_val, zero_out, scalar_members, selective)
+        d_blk = torch.from_numpy(np.frombuffer(blocks.tobytes(), dtype=np.uint8).copy()).cuda()
+        d_q = torch.empty(max(1, n * area), dtype=torch.int16, device='cuda')
+        d_reco = torch.empty(max(1, n * area), dtype=torch.int16, device='cuda') if want_reco else None
+        d_res = torch.empty(max(1, n * 32), dtype=torch.uint8, device='cuda'); d_nr = torch.empty(max(1, n), dtype=torch.uint8, device='cuda')
+        torch.cuda.synchronize()
+        self._chk(self.lib.vvb_tu_roundtrip_rdo_planes_dev(self.h, ctypes.byref(par), ctypes.byref(tq), org_plane, pred_plane, d_blk.data_ptr(), n, d_q.data_ptr(),
+                                                           d_reco.data_ptr() if want_reco else None, d_res.data_ptr(), d_nr.data_ptr()))
+        self.synchronize()
+        return dict(q=d_q.cpu().numpy()[:n * area].reshape(n, par.h, par.w), reco=d_reco.cpu().numpy()[:n * area].reshape(n, par.h, par.w) if want_reco else None,
+                    res=np.frombuffer(d_res.cpu().numpy().tobytes(), dtype=L.TU_RESULT_DT)[:n].copy(), need_rdoq=d_nr.cpu().numpy()[:n])
+
     # ---- MCTF
     def mctf_error_batch(self, org_plane, ref_plane, cands, low_res_filter=False):
         cands = np.ascontiguousarray(cands, dtype=L.MCTF_DT)

@@ -510,15 +510,16 @@ template<int LW> __device__ __forceinline__ auto org_pred_words( const int16_t* 
 enum ResiMode { RESI_POOL = 0, RESI_PLANES = 1, RESI_TWO_POOLS = 2 };
 
 // SRC = RESI_POOL: the residual of TU i is resi[i] of a compact pool [n][H][W].  SRC = RESI_PLANES: it is formed at load time, TU i sits at (blocks[i].x,
-// blocks[i].y) of orgPlane, its prediction at (+start_x, +start_y) of predPlane -- no compact residual buffer, no extra launch
+// blocks[i].y) of orgPlane, its prediction at (+start_x, +start_y) of predPlane -- no compact residual buffer, no extra launch.  SRC = RESI_TWO_POOLS: it is
+// formed at load time from the original pool resi[i] and the prediction pool pred[i]
 template<int LW, int LH, bool EXT, int SRC>
 __global__ void __launch_bounds__( 128 ) fwd_trquant_kernel( const __grid_constant__ TuPar par, const int8_t* __restrict__ trTable, const int32_t* __restrict__ scanTab,
-                                                             const int16_t* __restrict__ resi, const __grid_constant__ Plane orgPlane, const __grid_constant__ Plane predPlane,
+                                                             const int16_t* __restrict__ resi, const int16_t* __restrict__ pred,
+                                                             const __grid_constant__ Plane orgPlane, const __grid_constant__ Plane predPlane,
                                                              const vvb_block* __restrict__ blocks, int n,
                                                              int32_t* __restrict__ coefOut, int16_t* __restrict__ qOut, int32_t* __restrict__ absSumOut,
                                                              int32_t* __restrict__ lastPosOut, uint8_t* __restrict__ needRdoqOut )
 {
-  static_assert( SRC == RESI_POOL || SRC == RESI_PLANES, "the CUDA-core forward reads one pool or two planes" );
   using S = TuShape<LW, LH>;
   extern __shared__ __align__( 16 ) uint32_t smem[];
   constexpr int T = S::T, NTEAMS = S::NTEAMS;
@@ -543,6 +544,11 @@ __global__ void __launch_bounds__( 128 ) fwd_trquant_kernel( const __grid_consta
       pos = team_forward<LW, LH, EXT>( par, MtH, MtV, v, scanTab, tt, live,
                                        org_pred_words<LW>( orgPlane.origin + (ptrdiff_t) blk.y * so + blk.x, so,
                                                            predPlane.origin + (ptrdiff_t)( blk.y + blk.start_y ) * sp + blk.x + blk.start_x, sp ) );
+    }
+    else if constexpr( SRC == RESI_TWO_POOLS )
+    {
+      const size_t off = (size_t)( live ? tu : 0 ) * S::W * S::H;
+      pos = team_forward<LW, LH, EXT>( par, MtH, MtV, v, scanTab, tt, live, org_pred_words<LW>( resi + off, S::W, pred + off, S::W ) );
     }
     else
     {
