@@ -285,6 +285,9 @@ int vvb_scan_order( int w, int h, int32_t* out );
  *                   DepQuant.cpp:956-966; DepQuantX86.h:86-93, 163-166 adds the level capped to 126 / 127).  0 (default) follows the x86 members the encoder
  *                   installs on this platform, 1 the scalar ones of --SIMD=SCALAR.  Below 128 they agree.
  * The quantiser constants of Quantizer::initQuantBlock (:533-572) are derived inside from (w, h, bit_depth, qp, lambda) in the same double-precision steps.
+ * Any par->qp is accepted: the internal QP qp + 6 * (bit_depth - 8) is clipped to 0..63 + 6 * (bit_depth - 8) as QpParam does (Quant.cpp:109) and as the other
+ * entries and the dequantiser of dep_quant do, so the trellis runs at that clipped QP + 1.  Lambdas for which the reference's (uint32_t)( nomDistFactor * qScale2 )
+ * (DepQuant.cpp:566, = 2^nomDShift / lambda) reaches 2^32 have no defined result there, and none here.
  * par->lfnst_idx > 0 restricts the first tested position to 7 / 15 (:1164-1167).  need_rdoq (nullable, [n]): TUs with need_rdoq[i] == 0 return all-zero levels and
  * last_pos -1 (picture->useSelectiveRdoq, :1464-1468).  coef: [n][h][w] TCoeff as vvb_fwd_trquant returns them; q: [n][h][w] levels; abs_sum, last_pos nullable. */
 typedef struct { int32_t last_bits_x[32], last_bits_y[32], sig_sbb_bits[2][2], sig_bits[3][12][2], gtx_bits[21][6]; } vvb_dq_rates;   /* 1064 bytes */
@@ -316,7 +319,12 @@ int vvb_dep_quant_constants( const vvb_tu_par* par, const vvb_dq_par* dq, int64_
  * Uses par->{w, h, bit_depth, qp, is_chroma, sign_hiding, lfnst_idx}: lfnst_idx > 0 (the CU's index, whatever the component: :552-559) limits the scan to group 0 and,
  * for 4x4 / 8x8, to position 7.  The error scale of xSetErrScaleCoeffNoScalingList (:203-219) is derived inside in the same double-precision steps.
  * need_rdoq (nullable, [n]): TUs with need_rdoq[i] == 0 return all-zero levels (picture->useSelectiveRdoq, :273, 291-295).  coef: [n][h][w] TCoeff as vvb_fwd_trquant
- * returns them; q: [n][h][w] levels; abs_sum / last_pos (nullable) as uiAbsSum / tu.lastPos are left (last_pos -1 where the routine does not write it: nothing coded). */
+ * returns them; q: [n][h][w] levels; abs_sum / last_pos (nullable) as uiAbsSum / tu.lastPos are left (last_pos -1 where the routine does not write it: nothing coded).
+ * Levels above 32767 (reachable at the lowest QPs: up to 104858 in a 64-sided TU at internal QP 0) are stored into q as the member stores them into TCoeffSig
+ * (:942), i.e. as their low 16 bits, and the context templates read them as the member does.  One known difference remains, in engine 1 only, for levels from
+ * 65533 up (lowest QP of 64-sided TUs): the member adds a neighbour's template term from the full level and removes it (group zero-out, last-position choice,
+ * sign hiding) from abs() of the stored TCoeffSig, so a level whose low 16 bits are 0..3 or 65533..65535 leaves a term engine 1, which reads the stored levels
+ * only, cannot reconstruct.  Engine 2 keeps the member's add / remove bookkeeping and agrees there too. */
 typedef struct { int32_t sig_bits[12][2], par_bits[21][2], gt1_bits[21][2], gt2_bits[21][2], sig_group_bits[2][2], last_bits_x[16], last_bits_y[16], cbf_bits[2], pad[2]; } vvb_rdoq_rates;   /* 760 bytes */
 typedef struct { double lambda; int32_t thr_val, sbt_zero_out, pad[2]; } vvb_rdoq_par;
 int vvb_rdoq    ( vvb_ctx* ctx, const vvb_tu_par* par, const vvb_rdoq_par* rq, const vvb_rdoq_rates* rates, const int32_t* coef, const uint8_t* need_rdoq, int n,
@@ -324,7 +332,8 @@ int vvb_rdoq    ( vvb_ctx* ctx, const vvb_tu_par* par, const vvb_rdoq_par* rq, c
 int vvb_rdoq_dev( vvb_ctx* ctx, const vvb_tu_par* par, const vvb_rdoq_par* rq, const vvb_rdoq_rates* rates, const int32_t* dev_coef, const uint8_t* dev_need_rdoq, int n,
                   int16_t* dev_q, int32_t* dev_abs_sum, int32_t* dev_last_pos );
 /* kernel of vvb_rdoq: 1 (default) = the template of a position is gathered from its five neighbours when the position is visited; 2 = the templates are accumulated in the level slots of the
- * positions not visited yet (what the reference's m_tplBuf bookkeeping does) and lambda * bits of the frequent cases comes from per-call tables.  Same results. */
+ * positions not visited yet (what the reference's m_tplBuf bookkeeping does) and lambda * bits of the frequent cases comes from per-call tables.  Same results, but for
+ * the levels from 65533 up described above. */
 int vvb_set_rdoq_engine( vvb_ctx* ctx, int engine );
 /* the constants the call derives (no device needed): out = quantScale, errScale, qBits, useThres, remRegBins, numCG, firstScanPos (QuantRDOQ2.cpp:518-559, 573-583) */
 int vvb_rdoq_constants( const vvb_tu_par* par, const vvb_rdoq_par* rq, int32_t out[7] );

@@ -51,4 +51,18 @@ for (w, h) in ([(4, 4), (8, 8), (16, 16), (32, 32), (64, 64), (4, 32), (64, 4), 
             q = np.zeros((cnt, h, w), np.int16); s = np.zeros(cnt, np.int32)
             assert L.orc_rdoq_ts(w, h, 10, int(rs.choice([0, 17, 32, 51, 63])), 0, 57.3, P(tr), P(coef), cnt, P(q), P(s)) == 0
             assert L.orc_rdoq_bdpcm(w, h, 10, int(rs.choice([0, 17, 32, 51, 63])), 0, 1 + int(rs.randint(2)), 57.3, P(tr), P(coef), cnt, P(q), P(s)) == 0; n += 2 * cnt
+# DepQuant at the ends of the QP range, below the floor -6 * (bd - 8) and above 63 included (the clip of the internal QP keeps the scale index in range), both
+# member flavours, the lambdas the encoder derives there (only where the reference's uint32_t conversion is defined)
+from test_gpu_quant_limits import qp_ends, lambdas, dq_defined
+for (w, h) in ([(4, 4), (8, 8), (16, 16), (32, 32), (64, 64), (8, 4), (4, 32), (64, 16)] if WHAT == 'dq' else []):
+    for bd in (8, 10):
+        for qp in qp_ends(bd):
+            for lam in lambdas(qp, bd):
+                if not dq_defined(w, h, bd, qp, lam): continue
+                cnt = 4
+                coef = rs.choice([-32768, -3000, -1, 0, 0, 1, 400, 32767], size=(cnt, h, w)).astype(np.int32); coef[:, :, 32:] = 0; coef[:, 32:, :] = 0
+                rates = np.ascontiguousarray(g5['rates'][int(rs.randint(len(g5['rates'])))])
+                for scalar in (0, 1):
+                    q = np.zeros((cnt, h, w), np.int16); s = np.zeros(cnt, np.int32); l = np.zeros(cnt, np.int32)
+                    assert L.orc_dep_quant(w, h, bd, qp, lam, 8, 0, 0, scalar, P(rates), P(coef), cnt, P(q), P(s), P(l)) == 0; n += cnt
 print('SANITIZER CLEAN', n)

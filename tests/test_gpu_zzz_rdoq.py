@@ -101,7 +101,7 @@ def test_rdoq_binding_on_the_real_library():
 
 
 @pytest.mark.skipif(not os.path.exists(os.path.join(ROOT, 'oracle', '_ref', 'enc_identity')), reason='oracle/_ref/enc_identity not built')
-@pytest.mark.parametrize("W,H,F,preset,qp", [(80, 44, 4, 0, 37), (176, 144, 3, 0, 27), pytest.param(416, 240, 8, 0, 37, marks=first_hardware_run)])       # the last one is BASELINE configs[0] (added after the hardware run of the first two)
+@pytest.mark.parametrize("W,H,F,preset,qp", [(80, 44, 4, 0, 37), (176, 144, 3, 0, 27), (416, 240, 8, 0, 37)])       # the last one is BASELINE configs[0]
 def test_bitstream_identity_with_the_rdoq_seam_on_the_gpu(tmp_path, W, H, F, preset, qp):
     import vvenc_b200._lib as VL
     from test_encoder_identity import _identity_rdoq
@@ -133,9 +133,7 @@ def test_bitstream_identity_with_the_mctf_errors_on_the_gpu(tmp_path, W, H, F, p
     print('encoder identity with the MCTF errors on the GPU:', W, H, F, preset, kb)
 
 
-@first_hardware_run
-# ---- transform-skipped TUs: QuantRDOQ::rateDistOptQuantTS (vvb_rdoq_ts).  First hardware run of this entry point is the round-end suite: the shared text is pinned on the
-#      CPU exactly like the RDOQ above, the kernel wrapper has the shape of rdoq_kernel.
+# ---- transform-skipped TUs: QuantRDOQ::rateDistOptQuantTS (vvb_rdoq_ts)
 def test_gpu_rdoq_ts_golden(gpu, golden_rdoq):
     g = golden_rdoq
     rows = C.rdoq_ts_cases()
@@ -151,7 +149,6 @@ def test_gpu_rdoq_ts_golden(gpu, golden_rdoq):
     assert nonzero > 80
 
 
-@first_hardware_run
 def test_gpu_rdoq_ts_batches_vs_oracle(gpu, golden_rdoq):
     from _libs import dq_oracle, P
     O = dq_oracle()
@@ -175,7 +172,6 @@ def test_gpu_rdoq_ts_batches_vs_oracle(gpu, golden_rdoq):
         assert np.array_equal(r['abs_sum'], s) and (s > 0).sum() > n // 8, (w, h, int((s > 0).sum()))
 
 
-@first_hardware_run
 @pytest.mark.skipif(not os.path.exists(os.path.join(ROOT, 'oracle', '_ref', 'enc_identity')), reason='oracle/_ref/enc_identity not built')
 @pytest.mark.parametrize("W,H,F,preset,qp,min_ts", [(80, 44, 4, 0, 32, 40), (176, 144, 3, 0, 27, 1000)])
 def test_bitstream_identity_with_transform_skip_rdoq_on_the_gpu(tmp_path, W, H, F, preset, qp, min_ts):
@@ -185,7 +181,6 @@ def test_bitstream_identity_with_transform_skip_rdoq_on_the_gpu(tmp_path, W, H, 
     print('encoder identity with the transform-skip RDOQ on the GPU:', W, H, F, preset, kb)
 
 
-@first_hardware_run
 @pytest.mark.skipif(not have_ref(), reason='oracle/_ref not built')
 def test_rdoq_ts_binding_on_the_real_library():
     """rateDistOptQuantTSB200 (integration/TrQuantB200.h) bound to libvvenc_b200.so next to QuantRDOQ::rateDistOptQuantTS called as a member"""
@@ -197,7 +192,6 @@ def test_rdoq_ts_binding_on_the_real_library():
 
 
 # ---- BDPCM TUs: QuantRDOQ::forwardRDPCM (vvb_rdoq_bdpcm); inverse side = host running sums + vvb_inv_trquant of skipped transforms (verified kernel)
-@first_hardware_run
 def test_gpu_rdoq_bdpcm_golden(gpu, golden_rdoq):
     g = golden_rdoq
     rows = C.rdoq_ts_cases()
@@ -212,7 +206,6 @@ def test_gpu_rdoq_bdpcm_golden(gpu, golden_rdoq):
     assert nonzero > 70
 
 
-@first_hardware_run
 def test_gpu_rdoq_bdpcm_batches_vs_oracle(gpu, golden_rdoq):
     from _libs import dq_oracle, P
     O = dq_oracle()
@@ -233,7 +226,6 @@ def test_gpu_rdoq_bdpcm_batches_vs_oracle(gpu, golden_rdoq):
         assert np.array_equal(r['abs_sum'], s) and (s > 0).sum() > n // 10, (w, h, int((s > 0).sum()))
 
 
-@first_hardware_run
 @pytest.mark.skipif(not os.path.exists(os.path.join(ROOT, 'oracle', '_ref', 'enc_identity')), reason='oracle/_ref/enc_identity not built')
 @pytest.mark.parametrize("W,H,F,preset,qp,min_bdpcm", [(80, 44, 4, 0, 32, 100), (176, 144, 3, 0, 27, 2000)])
 def test_bitstream_identity_with_bdpcm_on_the_gpu(tmp_path, W, H, F, preset, qp, min_bdpcm):
@@ -243,7 +235,6 @@ def test_bitstream_identity_with_bdpcm_on_the_gpu(tmp_path, W, H, F, preset, qp,
     print('encoder identity with BDPCM on the GPU:', W, H, F, preset, kb)
 
 
-@first_hardware_run
 @pytest.mark.skipif(not have_ref(), reason='oracle/_ref not built')
 def test_rdoq_bdpcm_binding_on_the_real_library():
     """forwardRDPCMB200 next to QuantRDOQ::forwardRDPCM, and the inverse path of the BDPCM levels through invTransformNxNB200 next to TrQuant::invTransformNxN"""
@@ -255,7 +246,6 @@ def test_rdoq_bdpcm_binding_on_the_real_library():
 
 
 # ---- second engine of vvb_rdoq (vvb_set_rdoq_engine 2: accumulated templates + cost tables; rq_quant_tu_v2 is pinned on the CPU against the member like the first engine)
-@first_hardware_run
 def test_gpu_rdoq_second_engine_vs_golden_and_first_engine(gpu, golden_rdoq):
     from _libs import dq_oracle, P
     O = dq_oracle()

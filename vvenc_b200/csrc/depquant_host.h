@@ -130,11 +130,14 @@ inline void dq_build_tables( std::vector<DqScanInfo>& scanInfo, std::vector<DqNb
     }
 }
 
-// Quantizer::initQuantBlock (:533-572) for a luma, non-transform-skip TU without scaling lists.  qpInternal = cQP.Qp( false ) (CU QP + 6 * (bitDepth - 8)).
+// Quantizer::initQuantBlock (:533-572) for a luma, non-transform-skip TU without scaling lists.  qpInternal = CU QP + 6 * (bitDepth - 8), clipped here to
+// 0..63 + 6 * (bitDepth - 8) as QpParam clips cQP.Qp( false ) (Quant.cpp:109): below 0 the scale index qpRem would be negative.
 // Same double-precision operation order as the reference (the library is built with -ffp-contract=off; this file must be, too).
 inline DqQuant dq_init_quant( int w, int h, int bitDepth, int qpInternal, double lambda, int dqThrVal )
 {
   static const int quantScales[2][6] = { { 26214, 23302, 20560, 18396, 16384, 14564 }, { 18396, 16384, 14564, 13107, 11651, 10280 } };      // g_quantScales, Rom.cpp:1390-1394
+  const int maxQp = 63 + 6 * ( bitDepth - 8 );
+  qpInternal = qpInternal < 0 ? 0 : qpInternal > maxQp ? maxQp : qpInternal;
   int lw = 0, lh = 0;
   while( ( 1 << lw ) < w ) lw++;
   while( ( 1 << lh ) < h ) lh++;

@@ -223,7 +223,9 @@ VVB_HD void rq_quant_tu( const RqPar& P, const RqRates& R, const int32_t* scan, 
         if( spos != lastPosNow )                            // sigCtxIdAbsWithAcc( iScanPos, 0 ), ContextModelling.h:158-178
         {
           int numPos = 0, sumAbs = 0;
-#define RQ_UPD( v ) { const int a_ = ( v ); sumAbs += rq_min( 4 + ( a_ & 1 ), a_ ); numPos += a_ != 0; }
+          // the member accumulates min( 4 + ( level & 1 ), level ) of the full level (:950); a level above 32767 is kept here as its low 16 bits (TCoeffSig,
+          // :942), which read as uint16 give the same term for every level below 65533 (levels reach 104858 at the lowest QP of a 64-sided TU; the header states the rest)
+#define RQ_UPD( v ) { const int a_ = (uint16_t)( v ); sumAbs += rq_min( 4 + ( a_ & 1 ), a_ ); numPos += a_ != 0; }
           VVB_RQ_TEMPLATE( q, W, H, posX, posY, RQ_UPD )
 #undef RQ_UPD
           const int diag = posX + posY;
@@ -245,8 +247,8 @@ VVB_HD void rq_quant_tu( const RqPar& P, const RqRates& R, const int32_t* scan, 
 
         if( remRegBins < 4 )                                      // :731-736
         {
-          int sum = 0;
-#define RQ_SUM( v ) { sum += ( v ); }
+          int sum = 0;      // templateAbsSum sums abs() of the stored TCoeffSig (ContextModelling.h:242-265): a level from 32768 to 65535 is stored negative
+#define RQ_SUM( v ) { sum += rq_abs( v ); }
           VVB_RQ_TEMPLATE( q, W, H, posX, posY, RQ_SUM )
 #undef RQ_SUM
           const int sumAbs = rq_max( rq_min( sum, 31 ), 0 );      // templateAbsSum( ., ., 0 )
@@ -281,7 +283,7 @@ VVB_HD void rq_quant_tu( const RqPar& P, const RqRates& R, const int32_t* scan, 
           if( remRegBins >= 4 && spos != lastPosNow && lvlUp >= 4 )     // :777-781
           {
             int sum = 0;
-#define RQ_SUM( v ) { sum += ( v ); }
+#define RQ_SUM( v ) { sum += rq_abs( v ); }
             VVB_RQ_TEMPLATE( q, W, H, posX, posY, RQ_SUM )
 #undef RQ_SUM
             rice = c_rqGoRicePars[rq_max( rq_min( sum - 5 * 4, 31 ), 0 )];
@@ -564,6 +566,7 @@ struct RqCost
   int64_t sig[12][2];                // xiGetICost( sigBits[ctx][bin] )
   int64_t lvl[21][3];                // xiGetICRateCost( 1 / 2 / 3, ... ) with remRegBins >= 4 for greater-1 / parity / greater-2 context offset ctx
 };
+// the member adds the term of the full level when it decides one (:950) and removes min( 4 + ( a & 1 ), a ) of a = abs( TCoeffSig ) of the stored one (:1016, 1088, 1157)
 #define VVB_RQ_ENC( L ) ( ( L ) ? 32 + rq_min( 4 + ( ( L ) & 1 ), ( L ) ) : 0 )
 // add `delta` to the accumulators of the unvisited dependents of (x, y): every dependent when ALL is set (the position itself is being visited: everything to its left /
 // above is still ahead), else only those in groups that come earlier in the scan than group `curCG`
@@ -676,8 +679,8 @@ VVB_HD void rq_quant_tu_v2( const RqPar& P, const RqRates& R, const RqCost& C, c
 
         if( remRegBins < 4 )                                      // :731-736
         {
-          int sum = 0;
-#define RQ_SUM( v ) { sum += ( v ); }
+          int sum = 0;      // templateAbsSum sums abs() of the stored TCoeffSig (ContextModelling.h:242-265): a level from 32768 to 65535 is stored negative
+#define RQ_SUM( v ) { sum += rq_abs( v ); }
           VVB_RQ_TEMPLATE( q, W, H, posX, posY, RQ_SUM )
 #undef RQ_SUM
           const int sumAbs = rq_max( rq_min( sum, 31 ), 0 );      // templateAbsSum( ., ., 0 )
@@ -712,7 +715,7 @@ VVB_HD void rq_quant_tu_v2( const RqPar& P, const RqRates& R, const RqCost& C, c
           if( remRegBins >= 4 && spos != lastPosNow && lvlUp >= 4 )     // :777-781
           {
             int sum = 0;
-#define RQ_SUM( v ) { sum += ( v ); }
+#define RQ_SUM( v ) { sum += rq_abs( v ); }
             VVB_RQ_TEMPLATE( q, W, H, posX, posY, RQ_SUM )
 #undef RQ_SUM
             rice = c_rqGoRicePars[rq_max( rq_min( sum - 5 * 4, 31 ), 0 )];
@@ -863,7 +866,7 @@ VVB_HD void rq_quant_tu_v2( const RqPar& P, const RqRates& R, const RqCost& C, c
               {
                 const int rs_ = scan[grp * grpLen + p], px_ = rs_ & ( P.regionW - 1 ), py_ = rs_ >> lrw;
                 const int bp_ = ( py_ << lw ) + px_;
-                if( q[bp_] ) { const int enc_ = -VVB_RQ_ENC( (int) q[bp_] ); VVB_RQ_DEPS( q, W, px_, py_, enc_, false, cgIdx, widthInGroups, grp ) q[bp_] = 0; }      // remAbsVal1stPass
+                if( q[bp_] ) { const int enc_ = -VVB_RQ_ENC( rq_abs( (int) q[bp_] ) ); VVB_RQ_DEPS( q, W, px_, py_, enc_, false, cgIdx, widthInGroups, grp ) q[bp_] = 0; }      // remAbsVal1stPass
               }
               sumGrp = 0;
               if( lastGrp == grp ) { codedGrp = 0; uncodedGrp = 0; lastPosNow = -1; lastGrp = -1; }
@@ -913,7 +916,7 @@ VVB_HD void rq_quant_tu_v2( const RqPar& P, const RqRates& R, const RqCost& C, c
         {
           const int rs_ = scan[sp], px_ = rs_ & ( P.regionW - 1 ), py_ = rs_ >> lrw;
           const int bp_ = ( py_ << lw ) + px_;
-          if( q[bp_] ) { const int enc_ = -VVB_RQ_ENC( (int) q[bp_] ); VVB_RQ_DEPS( q, W, px_, py_, enc_, false, cgIdx, widthInGroups, grp ) q[bp_] = 0; }
+          if( q[bp_] ) { const int enc_ = -VVB_RQ_ENC( rq_abs( (int) q[bp_] ) ); VVB_RQ_DEPS( q, W, px_, py_, enc_, false, cgIdx, widthInGroups, grp ) q[bp_] = 0; }
         }
         lastPosNow = bestEnd - 1;
       }
@@ -953,7 +956,7 @@ VVB_HD void rq_quant_tu_v2( const RqPar& P, const RqRates& R, const RqCost& C, c
               if( flipDelta[n] < minDelta ) { minDelta = flipDelta[n]; minAt = n; }
             const int rs_ = scan[minAt + grpBase], px_ = rs_ & ( P.regionW - 1 ), py_ = rs_ >> lrw;
             const int bp = ( py_ << lw ) + px_;
-            const int encDelta_ = VVB_RQ_ENC( (int) q[bp] + flipStep[minAt] ) - VVB_RQ_ENC( (int) q[bp] );
+            const int encDelta_ = VVB_RQ_ENC( rq_abs( (int)(int16_t)( q[bp] + flipStep[minAt] ) ) ) - VVB_RQ_ENC( rq_abs( (int) q[bp] ) );   // :1157-1161, on the TCoeffSig
             if( encDelta_ ) VVB_RQ_DEPS( q, W, px_, py_, encDelta_, false, cgIdx, widthInGroups, grp )
             q[bp] = (int16_t)( q[bp] + flipStep[minAt] );
             sumGrp   += flipStep[minAt];
