@@ -190,6 +190,42 @@ int vvb_cost_pattern_dev( vvb_ctx* ctx, int dfunc, int org_plane, int ref_plane,
 /* device-side chaining: blocks[i].start = best[i].(dx,dy) (start of a refinement pattern / offset of the prediction block) */
 int vvb_blocks_set_start_dev( vvb_ctx* ctx, vvb_block* dev_blocks, const vvb_best* dev_best, int n );
 
+/* TZ integer motion search on the device = InterSearch::xTZSearch (EncoderLib/InterSearch.cpp:2297-2573) for every PU of a call, one PU shape per call
+ * (w, h in 4..128, powers of two, no larger than tz->ctu_size).  The whole walk runs per PU: start vector and zero vector, the extra start candidates, the search range around the best
+ * vector after them, integer early termination, the doubling diamond with its first-search stop, the zero-neighbourhood test, the adaptive or fixed raster,
+ * star refinement with its stop rule -- with xTZSearchHelp's strict `<` and its uiBestRound / ucPointNr / uiBestDistance bookkeeping, so the results equal
+ * the member's bit for bit.  The clipping that depends on the walk happens on the device: xClipMvSearch of the start vector and of every candidate
+ * (:2329-2331, :2357-2358) and xSetSearchRange around the best vector (:2372-2377).  Costs are 64-bit; the MV rate is the table of `me` (lambda, cost_scale,
+ * imv_shift); me->sub_shift is ignored, tz->sub_shift_mode selects the row sub-sampling per shape as RdCost::setDistParam does (RdCost.cpp:185-200).
+ * Reads are not clamped: every position the walk can read lies in the box xClipMvSearch allows, i.e. columns -(ctu_size + 7) .. pic_w + w + 6 and rows
+ * -(ctu_size + 7) .. pic_h + h + 6 around sample (0, 0), and a call whose ref_plane margin does not cover that box returns VVB_ERR_UNSUPPORTED.
+ * Errors: null pointers, negative counts, settings out of range, and (host-buffer call) PUs outside the picture or candidate ranges outside cands: VVB_ERR_ARG;
+ * shapes outside the domain (a PU larger than the CTU included), planes above 12 bits, an original plane smaller than the picture or a too small reference margin: VVB_ERR_UNSUPPORTED.
+ * The _dev twin cannot check PU positions and candidate ranges on the host: such a PU gets cost = sad = ~0 and best_distance = 0xffffffff. */
+typedef struct
+{
+  int32_t x, y;                    /* PU position in the original plane (inside the picture)                                                           */
+  int32_t start_hor, start_ver;    /* rcMv as xTZSearch receives it: internal units (1/16 pel), not clipped                                            */
+  int16_t pred_hor, pred_ver;      /* RdCost::setPredictor, quarter pel (as vvb_block.pred_*)                                                          */
+  int32_t cand_first, cand_count;  /* extra start candidates cands[cand_first .. +cand_count): m_BlkUniMvInfoBuffer's uniMvs[refPicList][iRefIdxPred]
+                                      in the buffer's order (:2352-2370), internal units, not clipped                                                   */
+} vvb_tz_pu;                       /* 28 bytes */
+typedef struct
+{
+  int32_t search_range;            /* m_iSearchRange                                                                                                   */
+  int32_t extended, fast;          /* bExtendedSettings, bFastSettings                                                                                 */
+  int32_t integer_et;              /* m_pcEncCfg->m_bIntegerET                                                                                         */
+  int32_t first_search_stop;       /* m_pcEncCfg->m_bFastMEAssumingSmootherMVEnabled                                                                   */
+  int32_t sub_shift_mode;          /* TZSearchStruct::subShiftMode: 0, 1 or 2                                                                          */
+  int32_t pic_w, pic_h, ctu_size, ifp_lines;   /* pcv.lumaWidth, pcv.lumaHeight, pcv.maxCUSize (16..128), m_pcEncCfg->m_ifpLines                    */
+} vvb_tz_par;
+/* mv = rcMv as written out (integer pel); sad = ruiSAD (best cost minus its MV rate); cost = uiBestSad; best_distance = uiBestDistance at the end */
+typedef struct { int32_t mv_hor, mv_ver; uint64_t sad, cost; uint32_t best_distance, pad; } vvb_tz_best;   /* 32 bytes */
+int vvb_tz_search    ( vvb_ctx* ctx, int org_plane, int ref_plane, const vvb_tz_pu* pus, int n, int w, int h, const vvb_me_par* me, const vvb_tz_par* tz,
+                       const int32_t* cands /* [n_cands][2] hor, ver; nullable when n_cands == 0 */, int n_cands, vvb_tz_best* out );
+int vvb_tz_search_dev( vvb_ctx* ctx, int org_plane, int ref_plane, const vvb_tz_pu* dev_pus, int n, int w, int h, const vvb_me_par* me, const vvb_tz_par* tz,
+                       const int32_t* dev_cands, int n_cands, vvb_tz_best* dev_out );
+
 /* ---- forward transform + quantise (TrQuant::transformNxN; luma and chroma TUs with sides 4..64, transform skip included; ---------------
  * CommonLib/TrQuant.cpp:688-736 -> xT :481-564 -> Quant::quant CommonLib/Quant.cpp:735-833 -> QuantCore :132-230,
  * and Quant::xNeedRDOQ :835-891 -> needRdoqCore :264-278).  All TUs of a call share shape and transform types.

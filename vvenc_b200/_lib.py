@@ -26,6 +26,10 @@ class vvb_me_par(ctypes.Structure):
     _fields_ = [('lam', ctypes.c_double), ('cost_scale', ctypes.c_int32), ('imv_shift', ctypes.c_int32), ('sub_shift', ctypes.c_int32), ('quad_order', ctypes.c_int32), ('pattern_radius', ctypes.c_int32), ('pad', ctypes.c_int32)]
 
 
+class vvb_tz_par(ctypes.Structure):
+    _fields_ = [(k, ctypes.c_int32) for k in ('search_range', 'extended', 'fast', 'integer_et', 'first_search_stop', 'sub_shift_mode', 'pic_w', 'pic_h', 'ctu_size', 'ifp_lines')]
+
+
 class vvb_tu_par(ctypes.Structure):
     _fields_ = [('w', ctypes.c_int32), ('h', ctypes.c_int32), ('tr_hor', ctypes.c_int32), ('tr_ver', ctypes.c_int32), ('bit_depth', ctypes.c_int32),
                 ('qp', ctypes.c_int32), ('is_irap', ctypes.c_int32), ('dep_quant', ctypes.c_int32), ('sign_hiding', ctypes.c_int32), ('lfnst_idx', ctypes.c_int32), ('lfnst_set', ctypes.c_int32), ('lfnst_transpose', ctypes.c_int32),
@@ -88,6 +92,9 @@ MV_DT = np.dtype([('dx', '<i2'), ('dy', '<i2')])
 TU_RESULT_DT = np.dtype([('dist_reco', '<u8'), ('dist_resi', '<u8'), ('dist_zero', '<u8'), ('abs_sum', '<i4'), ('last_pos', '<i4')])
 MCTF_MV_DT = np.dtype([('x', '<i4'), ('y', '<i4'), ('error', '<i4'), ('rmsme', '<u2'), ('pad', '<u2')])
 MCTF_DT = np.dtype([('x', '<i4'), ('y', '<i4'), ('mvx', '<i4'), ('mvy', '<i4'), ('w', '<u2'), ('h', '<u2')])
+TZ_PU_DT = np.dtype([('x', '<i4'), ('y', '<i4'), ('start_hor', '<i4'), ('start_ver', '<i4'), ('pred_hor', '<i2'), ('pred_ver', '<i2'), ('cand_first', '<i4'), ('cand_count', '<i4')])
+TZ_BEST_DT = np.dtype([('mv_hor', '<i4'), ('mv_ver', '<i4'), ('sad', '<u8'), ('cost', '<u8'), ('best_distance', '<u4'), ('pad', '<u4')])
+assert TZ_PU_DT.itemsize == 28 and TZ_BEST_DT.itemsize == 32
 assert CAND_DT.itemsize == 32 and BLOCK_DT.itemsize == 24 and BEST_DT.itemsize == 16 and MCTF_DT.itemsize == 20
 
 # every symbol include/vvenc_b200.h declares: name -> (restype, argtypes)
@@ -123,6 +130,8 @@ SYMBOLS = {
     'vvb_cost_pattern': (c_i, [c_p, c_i, c_i, c_i, c_p, c_i, c_i, c_i, c_p, c_i, ctypes.POINTER(vvb_me_par), c_p, c_p]),
     'vvb_cost_pattern_dev': (c_i, [c_p, c_i, c_i, c_i, c_p, c_i, c_i, c_i, c_p, c_i, ctypes.POINTER(vvb_me_par), c_p, c_p]),
     'vvb_blocks_set_start_dev': (c_i, [c_p, c_p, c_p, c_i]),
+    'vvb_tz_search': (c_i, [c_p, c_i, c_i, c_p, c_i, c_i, c_i, ctypes.POINTER(vvb_me_par), ctypes.POINTER(vvb_tz_par), c_p, c_i, c_p]),
+    'vvb_tz_search_dev': (c_i, [c_p, c_i, c_i, c_p, c_i, c_i, c_i, ctypes.POINTER(vvb_me_par), ctypes.POINTER(vvb_tz_par), c_p, c_i, c_p]),
     'vvb_fwd_trquant': (c_i, [c_p, ctypes.POINTER(vvb_tu_par), c_p, c_i, c_p, c_p, c_p, c_p, c_p]),
     'vvb_fwd_trquant_dev': (c_i, [c_p, ctypes.POINTER(vvb_tu_par), c_p, c_i, c_p, c_p, c_p, c_p, c_p]),
     'vvb_set_tensor_transform': (c_i, [c_p, c_i]),

@@ -5,7 +5,7 @@
 
   getDistPart-like single calls .... dist_block / sad_mask_block / sad_x5_block / fix_wsse_block   (RdCost.h:74-75,117)
   batched candidate evaluation ..... dist_batch (descriptor list), dist_pool (RDO candidate pools)
-  motion search .................... sad_search (xPatternSearch), sad_pattern (fixed TZ point set)
+  motion search .................... sad_search (xPatternSearch), sad_pattern (fixed TZ point set), tz_search (xTZSearch walk)
   TU coding ........................ fwd_trquant (TrQuant::transformNxN: xT + Quant::quant + xNeedRDOQ)
   pre-analysis ..................... mctf_error_batch (MCTF::motionErrorLuma)
   affine ME ........................ affine_sobel / affine_equal_coeff
@@ -202,6 +202,20 @@ class CostEngine:
         best = np.zeros(n, dtype=L.BEST_DT) if want_best else None
         self._chk(self.lib.vvb_sad_pattern(self.h, org_plane, ref_plane, _p(blocks), n, w, h, _p(pattern), K, ctypes.byref(par), _p(sad), _p(best)))
         return sad, best
+
+    @staticmethod
+    def tz_par(search_range, pic_w, pic_h, ctu_size, extended=False, fast=False, integer_et=False, first_search_stop=False, sub_shift_mode=0, ifp_lines=0):
+        return L.vvb_tz_par(search_range, int(extended), int(fast), int(integer_et), int(first_search_stop), sub_shift_mode, pic_w, pic_h, ctu_size, ifp_lines)
+
+    def tz_search(self, org_plane, ref_plane, pus, w, h, me, tz, cands=None):
+        """InterSearch::xTZSearch for every PU of one shape.  pus: TZ_PU_DT array; cands: int32 [n_cands][2] (hor, ver, 1/16 pel) the PUs' cand_first /
+        cand_count index into.  Returns a TZ_BEST_DT array (mv in integer pels, sad = ruiSAD, cost = uiBestSad, best_distance = uiBestDistance)."""
+        pus = np.ascontiguousarray(pus, dtype=L.TZ_PU_DT)
+        cands = np.zeros((0, 2), dtype=np.int32) if cands is None else np.ascontiguousarray(cands, dtype=np.int32).reshape(-1, 2)
+        out = np.zeros(len(pus), dtype=L.TZ_BEST_DT)
+        self._chk(self.lib.vvb_tz_search(self.h, org_plane, ref_plane, _p(pus), len(pus), w, h, ctypes.byref(me), ctypes.byref(tz),
+                                         _p(cands) if len(cands) else None, len(cands), _p(out)))
+        return out
 
     def cost_pattern(self, dfunc, org_plane, ref_plane, blocks, w, h, pattern, par, want_cost=True, want_best=True):
         """any distortion family over the fixed pattern (e.g. DF_HAD integer refinement around blocks['start_*'])"""

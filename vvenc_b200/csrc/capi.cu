@@ -21,6 +21,7 @@
 #include "rdoq_kernels.cuh"
 #include "batch_kernels.cuh"
 #include "mctf_control_kernels.cuh"
+#include "tz_kernels.cuh"
 #include "depquant_host.h"
 #include "rdoq_host.h"
 #include "vvc_tables.h"
@@ -1227,6 +1228,79 @@ int vvb_blocks_set_start_dev( vvb_ctx* ctx, vvb_block* dBlocks, const vvb_best* 
   blocks_set_start_kernel<<<std::min( ( n + 255 ) / 256, ctx->numSMs * 8 ), 256, 0, ctx->stream>>>( dBlocks, dBest, n );
   CHECK_LAUNCH( "blocks_set_start_kernel" );
   return VVB_OK;
+}
+
+// ---- TZ search (tz_kernels.cuh) ----------------------------------------------------------------------------------
+static int tzSetup( vvb_ctx* ctx, int orgPlane, int refPlane, int n, int w, int h, const vvb_me_par* me, const vvb_tz_par* tz, int nCands, TzPar& tp, MePar& mp )
+{
+  if( !me || !tz || n < 0 || nCands < 0 ) return fail( ctx, VVB_ERR_ARG, "bad arguments" );
+  if( !validPlane( ctx, orgPlane ) || !validPlane( ctx, refPlane ) ) return fail( ctx, VVB_ERR_ARG, "unknown plane" );
+  if( tz->search_range < 0 || tz->search_range > 4096 || tz->sub_shift_mode < 0 || tz->sub_shift_mode > 2 || tz->pic_w < 1 || tz->pic_h < 1 || tz->pic_w > 16384 ||
+      tz->pic_h > 16384 || !isPow2( tz->ctu_size ) || tz->ctu_size < 16 || tz->ctu_size > 128 || tz->ifp_lines < 0 || tz->ifp_lines > 1024 )
+    return fail( ctx, VVB_ERR_ARG, "TZ settings out of range (search_range 0..4096, sub_shift_mode 0..2, ctu_size 16..128, picture sides 1..16384)" );
+  if( !isPow2( w ) || !isPow2( h ) || w < 4 || h < 4 || w > 128 || h > 128 ) return fail( ctx, VVB_ERR_UNSUPPORTED, "TZ search PUs are 4..128 powers of two" );
+  // a PU lies inside its CTU; the margin rule below relies on it, because the ifp_lines bottom clip of a PU taller than the CTU rows it may reach would fall above
+  // the picture (xClipMvSearch's verMax below its verMin)
+  if( w > tz->ctu_size || h > tz->ctu_size ) return fail( ctx, VVB_ERR_UNSUPPORTED, "TZ search PUs no larger than the CTU" );
+  const Plane &op = ctx->planes.p[orgPlane], &rp = ctx->planes.p[refPlane];
+  if( op.bitDepth > 12 || rp.bitDepth > 12 ) return fail( ctx, VVB_ERR_UNSUPPORTED, "TZ search planes of up to 12 bits" );
+  if( w > tz->pic_w || h > tz->pic_h || op.width < tz->pic_w || op.height < tz->pic_h ) return fail( ctx, VVB_ERR_UNSUPPORTED, "the original plane or the picture is smaller than the PUs" );
+  // the box xClipMvSearch allows (InterSearch.cpp:2134-2152) plus the block: columns -(ctu + 7) .. pic_w + w + 6, rows likewise
+  const int need = std::max( tz->ctu_size + 7, std::max( tz->pic_w + w + 7 - rp.width, tz->pic_h + h + 7 - rp.height ) );
+  if( rp.margin < need ) return fail( ctx, VVB_ERR_UNSUPPORTED, "reference margin below the reach of the TZ clip rules (ctu_size + 7 left / top, w + 7 / h + 7 beyond the picture)" );
+  int rc = makeMePar( ctx, me, mp );
+  if( rc ) return rc;
+  int subShift = 0;
+  if( tz->sub_shift_mode == 1 && h > 8 && w <= 128 ) subShift = 1;        // RdCost::setDistParam (RdCost.cpp:185-200)
+  if( tz->sub_shift_mode == 2 && h > 8 ) subShift = 1;
+  mp.subShift = subShift;
+  tp.searchRange = tz->search_range; tp.extended = tz->extended != 0; tp.fast = tz->fast != 0; tp.integerET = tz->integer_et != 0;
+  tp.firstSearchStop = tz->first_search_stop != 0; tp.subShift = subShift;
+  tp.picW = tz->pic_w; tp.picH = tz->pic_h; tp.ctuSize = tz->ctu_size; tp.ctuLog2 = ilog2h( tz->ctu_size );
+  tp.heightInCtus = ( tz->pic_h + tz->ctu_size - 1 ) / tz->ctu_size; tp.ifpLines = tz->ifp_lines;
+  tp.w = w; tp.h = h; tp.nCands = nCands;
+  return VVB_OK;
+}
+
+int vvb_tz_search_dev( vvb_ctx* ctx, int orgPlane, int refPlane, const vvb_tz_pu* dPus, int n, int w, int h, const vvb_me_par* me, const vvb_tz_par* tz,
+                       const int32_t* dCands, int nCands, vvb_tz_best* dOut )
+{
+  if( !ctx || !dPus || !dOut || ( nCands > 0 && !dCands ) ) return fail( ctx, VVB_ERR_ARG, "bad arguments" );
+  TzPar tp; MePar mp;
+  int rc = tzSetup( ctx, orgPlane, refPlane, n, w, h, me, tz, nCands, tp, mp );
+  if( rc ) return rc;
+  if( n == 0 ) return VVB_OK;
+  CU( cudaSetDevice( ctx->device ) );
+  const int G = pick_group( FAM_SAD, w, h >> tp.subShift );
+  void ( *kernel )( const Plane, const Plane, const vvb_tz_pu*, int, const int32_t*, const TzPar, const MePar, vvb_tz_best* ) =
+    G == 4 ? tz_search_kernel<4> : G == 8 ? tz_search_kernel<8> : G == 16 ? tz_search_kernel<16> : tz_search_kernel<32>;
+  // persistent warps: as many CTAs as stay resident, each warp walks PUs i, i + warps, ...
+  const int perWarp = tz_warp_smem( w, h ), wpc = std::max( 1, std::min( 4, ( 48 * 1024 ) / perWarp ) );
+  const size_t smem = (size_t) wpc * perWarp;
+  int perSm = 0;
+  CU( cudaOccupancyMaxActiveBlocksPerMultiprocessor( &perSm, kernel, wpc * 32, smem ) );
+  const int grid = (int) std::min<long long>( ( n + wpc - 1 ) / wpc, (long long) ctx->numSMs * std::max( 1, perSm ) );
+  kernel<<<grid, wpc * 32, smem, ctx->stream>>>( ctx->planes.p[orgPlane], ctx->planes.p[refPlane], dPus, n, dCands, tp, mp, dOut );
+  CHECK_LAUNCH( "tz_search_kernel" );
+  return VVB_OK;
+}
+
+int vvb_tz_search( vvb_ctx* ctx, int orgPlane, int refPlane, const vvb_tz_pu* pus, int n, int w, int h, const vvb_me_par* me, const vvb_tz_par* tz,
+                   const int32_t* cands, int nCands, vvb_tz_best* out )
+{
+  if( !ctx || !pus || !out || ( nCands > 0 && !cands ) ) return fail( ctx, VVB_ERR_ARG, "bad arguments" );
+  TzPar tp; MePar mp;
+  int rc = tzSetup( ctx, orgPlane, refPlane, n, w, h, me, tz, nCands, tp, mp );
+  if( rc || n == 0 ) return rc;
+  for( int i = 0; i < n; i++ )
+  {
+    const vvb_tz_pu& p = pus[i];
+    if( p.x < 0 || p.y < 0 || p.x > tz->pic_w - w || p.y > tz->pic_h - h ) return fail( ctx, VVB_ERR_ARG, "PU outside the picture" );
+    if( p.cand_first < 0 || p.cand_count < 0 || p.cand_first > nCands - p.cand_count ) return fail( ctx, VVB_ERR_ARG, "candidate range outside cands" );
+  }
+  const vvb_tz_pu* dP; const int32_t* dC; vvb_tz_best* dO;
+  return HostCall( ctx ).in( dP, pus, n ).in( dC, cands, (size_t) 2 * nCands ).out( dO, out, n )
+                        .run( [&] { return vvb_tz_search_dev( ctx, orgPlane, refPlane, dP, n, w, h, me, tz, dC, nCands, dO ); } );
 }
 
 // ---- transform + quantise ----------------------------------------------------------------------------------------

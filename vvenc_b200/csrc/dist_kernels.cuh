@@ -19,7 +19,10 @@ enum { FAM_SSE = 0, FAM_SAD = 1, FAM_HAD = 2, FAM_HAD_FAST = 3, FAM_HAD_2SAD = 4
 // SAD: sum over rows y = 0, s, 2s.. (s = 1<<subShift) of sum_x |org - cur|, result << subShift
 // (CommonLib/RdCost.cpp:300-335; every width-specialised variant computes the same value)
 // ---------------------------------------------------------------------------------------------------------------
-template<int G>
+// SMEM: org points into shared memory (a block staged once and searched many times) and is read with plain loads
+template<bool SMEM, class T> __device__ __forceinline__ T org_load( const T* p ) { if constexpr( SMEM ) return *p; else return __ldg( p ); }
+
+template<int G, bool ORG_SMEM = false>
 __device__ __forceinline__ uint32_t group_sad( const int16_t* __restrict__ org, int so, const int16_t* __restrict__ cur, int sc,
                                                int w, int h, int subShift, int lg )
 {
@@ -34,7 +37,7 @@ __device__ __forceinline__ uint32_t group_sad( const int16_t* __restrict__ org, 
     for( int i = lg; i < total; i += G )
     {
       const int r = i >> lc, c = i & ( cpr - 1 ), y = r << subShift;
-      const uint4 a = __ldg( reinterpret_cast<const uint4*>( org + (size_t) y * so ) + c );
+      const uint4 a = org_load<ORG_SMEM>( reinterpret_cast<const uint4*>( org + (size_t) y * so ) + c );
       const uint4 b = __ldg( reinterpret_cast<const uint4*>( cur + (size_t) y * sc ) + c );
       acc = sad2_acc( a.x, b.x, acc ); acc = sad2_acc( a.y, b.y, acc );
       acc = sad2_acc( a.z, b.z, acc ); acc = sad2_acc( a.w, b.w, acc );
@@ -46,7 +49,7 @@ __device__ __forceinline__ uint32_t group_sad( const int16_t* __restrict__ org, 
     for( int i = lg; i < total; i += G )
     {
       const int r = i >> lc, c = i & ( cpr - 1 ), y = r << subShift;
-      const uint32_t a = __ldg( reinterpret_cast<const uint32_t*>( org + (size_t) y * so ) + c );
+      const uint32_t a = org_load<ORG_SMEM>( reinterpret_cast<const uint32_t*>( org + (size_t) y * so ) + c );
       const uint32_t b = __ldg( reinterpret_cast<const uint32_t*>( cur + (size_t) y * sc ) + c );
       acc = sad2_acc( a, b, acc );
     }
@@ -57,7 +60,7 @@ __device__ __forceinline__ uint32_t group_sad( const int16_t* __restrict__ org, 
     for( int i = lg; i < total; i += G )
     {
       const int r = i >> lw, x = i & ( w - 1 ), y = r << subShift;
-      acc += abs( (int) __ldg( org + (size_t) y * so + x ) - (int) __ldg( cur + (size_t) y * sc + x ) );
+      acc += abs( (int) org_load<ORG_SMEM>( org + (size_t) y * so + x ) - (int) __ldg( cur + (size_t) y * sc + x ) );
     }
   }
   return group_sum_u32<G>( (uint32_t) acc ) << subShift;
