@@ -417,7 +417,8 @@ int vvb_create( vvb_ctx** out, int device )
     smemLimit( sad_search_kernel<false, false>, 220 * 1024 ), smemLimit( sad_search_kernel<true, false>, 220 * 1024 ),
     smemLimit( sad_search_kernel<false, true>, 220 * 1024 ), smemLimit( sad_search_kernel<true, true>, 220 * 1024 ),
     smemLimit( sad_search_kernel<false, true, true>, 220 * 1024 ), smemLimit( sad_search_kernel<true, true, true>, 220 * 1024 ),
-    smemLimit( sad_pyramid8_kernel<2>, 227 * 1024 ), smemLimit( sad_pyramid8_kernel<3>, 227 * 1024 ), smemLimit( sad_pyramid8_kernel<4>, 227 * 1024 ),
+    smemLimit( sad_pyramid8_kernel<2, 0>, 227 * 1024 ), smemLimit( sad_pyramid8_kernel<3, 0>, 227 * 1024 ), smemLimit( sad_pyramid8_kernel<4, 0>, 227 * 1024 ),
+    smemLimit( sad_pyramid8_kernel<4, PYR_FIXED_N>, 227 * 1024 ),
     smemLimit( affine_eq_batch_kernel<4>, 100 * 1024 ), smemLimit( affine_eq_batch_kernel<6>, 100 * 1024 ),
     VVB_RING_SMEM( 16 ), VVB_RING_SMEM( 32 ), VVB_RING_SMEM( 64 ),
     smemLimit( mctf_error_packed_kernel, 100 * 1024 ), smemLimit( mctf_grid_kernel, 200 * 1024 ), smemLimit( mctf_wave_kernel, 100 * 1024 ),
@@ -967,9 +968,11 @@ static int pyramidV2LaunchLevel( vvb_ctx* ctx, int orgPlane, int refPlane, const
   static const int forced = []{ const char* e = getenv( "VVB_PYR_THREADS" ); return e ? atoi( e ) : 0; }();     // tuning aid: fixed CTA size
   if( forced >= 64 && forced <= maxT && ( forced & 31 ) == 0 ) bd = forced;
   // 64x64 roots fill an SM each: one CTA per SM walks a run of consecutive roots and carries the shared half of each window to its right neighbour.
-  // Smaller roots share SMs and keep one CTA per root.
+  // Smaller roots share SMs and keep one CTA per root.  A +-32 range (unclipped) runs the instantiation compiled for its geometry.
   const int runs = LV == 4 ? std::min( nRoots, ctx->numSMs ) : nRoots;
-  sad_pyramid8_kernel<LV><<<runs, bd, (size_t) L.total, ctx->stream>>>( ctx->planes.p[orgPlane], ctx->planes.p[refPlane], lv, rootFirst, nRoots, nx, ny, mp, L, 1u, 8u );
+  auto kernel = sad_pyramid8_kernel<LV, 0>;
+  if constexpr( LV == 4 ) { if( nx == PYR_FIXED_N && ny == PYR_FIXED_N ) kernel = sad_pyramid8_kernel<LV, PYR_FIXED_N>; }
+  kernel<<<runs, bd, (size_t) L.total, ctx->stream>>>( ctx->planes.p[orgPlane], ctx->planes.p[refPlane], lv, rootFirst, nRoots, nx, ny, mp, L, 1u, 8u );
   CHECK_LAUNCH( "sad_pyramid8_kernel" );
   return VVB_OK;
 }

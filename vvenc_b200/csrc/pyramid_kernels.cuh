@@ -27,7 +27,14 @@
 // the CTA copies the next window's new R pels of every row into a staging area with cp.async behind its own candidate loop (L2 prefetches cover the next
 // root's descriptors and originals), then shifts the kept half of its window left and drops the staged columns in instead of restaging it from global
 // memory.  The rate tables are staged once per CTA.  Any other next root (new row, other range, broken quad tree, 16-bit staging path, a staging area
-// that does not fit) is restaged in full, so every result is the one a CTA per root would give.
+// that does not fit) is restaged in full, so every result is the one a CTA per root would give.  The next root's originals are copied the same way into a
+// second originals buffer where it fits (16-byte aligned rows), whether or not the window carries.  The 32x32 tables are zeroed once per CTA and the argmin
+// pass clears each entry as it reads it, so no root spends a pass and a barrier on zeroing them; the prologue's row sums live in win1 until the shifted copy
+// is formed after the box sums.
+//
+// Geometry: sad_pyramid8_kernel<LV, 0> takes the range and the shared-memory layout from the launch; sad_pyramid8_kernel<4, PYR_FIXED_N> is compiled for a
+// 65 x 65 range (+-32, unclipped), where the window pitch, the table strides and the item counts are constants: row offsets fold into LDS immediates and the
+// item decode divides by constants instead of float reciprocals.
 #pragma once
 #include "search_kernels.cuh"
 
@@ -40,6 +47,7 @@ template<int LV> constexpr int pyr_max_threads() { return LV == 2 ? 640 : 512; }
 #define PYR_MVN         296                      // rate-table entries per strip slot: 0..79 real, the rest "never wins" (padded columns index 250 + row bits)
 #define PYR_PAD_BITS    250
 #define PYR_NEVER       ( 1u << 26 )             // cost no real candidate reaches; 4 * PYR_NEVER * 8 still fits 32 bits
+#define PYR_FIXED_N     65                       // range with a fixed-geometry instantiation of the 64x64 kernel: +-32, the encoder's default search range
 
 struct PyrLevels { const vvb_block* blocks[4]; vvb_best* best[4]; };
 
@@ -48,13 +56,14 @@ struct PyrSmem
   int nStrips, nxp, nyp, bStride, ws, winH, winWords, vRows, vPitch, nT, tStride;
   int offWin0, offWin1, offV, offOrg, offBits, offPred, offSumA, offKey32, offKey64, offMv8, offMvRaw, offT, offStage, total;   // bytes
   int stageWords;                                        // words of the row walk's staging area (winH rows of R / 2 words); 0: every root restages in full
+  int offOrgNext;                                        // bytes: second originals buffer the row walk fills for the next root behind the loop; 0: none
 };
 
 template<int LV>
-__host__ __device__ inline PyrSmem pyr_smem( int nx, int ny )
+__host__ __device__ constexpr PyrSmem pyr_smem( int nx, int ny )
 {
   constexpr int R = 8 << ( LV - 1 ), NB0 = 1 << ( 2 * ( LV - 1 ) ), NBLK = ( 4 * NB0 - 1 ) / 3;
-  PyrSmem s;
+  PyrSmem s{};
   s.nStrips = ( nx + 7 ) >> 3;
   s.nxp     = s.nStrips * 8;
   s.nyp     = ( ny + 1 + 7 ) & ~7;                       // row B of the last pair may be one past the range
@@ -84,8 +93,7 @@ __host__ __device__ inline PyrSmem pyr_smem( int nx, int ny )
   s.offOrg  = o;   o += R * R * 2;
   s.offBits = o;   o += NBLK * s.bStride;
   s.offT    = ( o + 15 ) & ~15;
-  const int tBytes = s.nT * s.tStride * 4, hsBytes = s.winH * s.vPitch * 2;      // the row-sum scratch of the prologue lives where the tables go later
-  s.total   = s.offT + ( tBytes > hsBytes ? tBytes : hsBytes ) + 16;
+  s.total   = s.offT + s.nT * s.tStride * 4 + 16;        // the prologue's row-sum scratch lives in win1 (ws > vPitch), which is written after it
   // row walk of 64x64 roots: the next root's new R pels of every window row are copied behind the candidate loop into the shared memory the rest leaves
   // free.  Where that does not fit (larger ranges), or a row holds more words than the carry's 4 per lane, the walk restages every root in full.
   s.offStage   = ( s.total + 15 ) & ~15;
@@ -94,6 +102,12 @@ __host__ __device__ inline PyrSmem pyr_smem( int nx, int ny )
   {
     s.stageWords = s.winH * ( R / 2 );
     s.total      = s.offStage + s.stageWords * 4;
+  }
+  // and the next root's originals go to a second buffer where that fits (at +-32 it does, next to the staging area)
+  if( LV == 4 && ( ( s.total + 15 ) & ~15 ) + R * R * 2 <= 227 * 1024 )
+  {
+    s.offOrgNext = ( s.total + 15 ) & ~15;
+    s.total      = s.offOrgNext + R * R * 2;
   }
   return s;
 }
@@ -153,19 +167,31 @@ __device__ __forceinline__ uint32_t pyr_finish_row( const int (&acc)[8], const u
   return bk;
 }
 
-template<int LV>
+// a / d for a >= 0, d >= 1: with the geometry fixed at compile time d is a constant and this is an integer division by a constant (a multiply-high); otherwise
+// the float reciprocal inv = 1 / d of the runtime count
+template<int NXY>
+__device__ __forceinline__ int pyr_div( int a, int d, float inv ) { return NXY ? (int)( (unsigned) a / (unsigned) d ) : div_rcp( a, inv ); }
+
+// NXY = 0: the range nx x ny and the layout L come from the launch.  NXY > 0: nx = ny = NXY, and the layout and every count derived from it are compile-time
+// constants, so window, box-sum and MV-bit offsets fold into the LDS immediates and the item decode needs no float reciprocals (the host checks that the
+// launch's range is NXY x NXY).
+template<int LV, int NXY>
 __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kernel( const __grid_constant__ Plane orgPlane, const __grid_constant__ Plane refPlane,
-                                                                             const __grid_constant__ PyrLevels lv, int rootFirst, int nRoots, int nx, int ny,
-                                                                             const __grid_constant__ MePar par, const __grid_constant__ PyrSmem L,   // L = pyr_smem<LV>( nx, ny )
+                                                                             const __grid_constant__ PyrLevels lv, int rootFirst, int nRoots, int nxArg, int nyArg,
+                                                                             const __grid_constant__ MePar par, const __grid_constant__ PyrSmem LArg,   // pyr_smem<LV>( nx, ny )
                                                                              uint32_t one, uint32_t eight )
 {
   constexpr int R = 8 << ( LV - 1 ), NB0 = 1 << ( 2 * ( LV - 1 ) ), NQ = NB0 / 4, NBLK = ( 4 * NB0 - 1 ) / 3, LTOP = LV - 1;
   constexpr int OFF1 = NB0, OFF2 = NB0 + NQ, OFF3 = NB0 + NQ + NQ / 4, NT = LV == 4 ? 4 : ( LV == 3 ? 1 : 0 );
+  constexpr PyrSmem LF = pyr_smem<LV>( NXY ? NXY : 1, NXY ? NXY : 1 );
+  const int nx = NXY ? NXY : nxArg, ny = NXY ? NXY : nyArg;
+  const PyrSmem L = NXY ? LF : LArg;
   extern __shared__ __align__( 128 ) unsigned char smemRaw[];
   uint32_t* win0w = reinterpret_cast<uint32_t*>( smemRaw + L.offWin0 );
   uint32_t* win1w = reinterpret_cast<uint32_t*>( smemRaw + L.offWin1 );
   uint16_t* V     = reinterpret_cast<uint16_t*>( smemRaw + L.offV );
   int16_t*  orgS  = reinterpret_cast<int16_t*>( smemRaw + L.offOrg );
+  int16_t*  orgN  = reinterpret_cast<int16_t*>( smemRaw + L.offOrgNext );      // the other originals buffer (L.offOrgNext > 0)
   unsigned char* bitsS = smemRaw + L.offBits;
   int2*     sPred = reinterpret_cast<int2*>( smemRaw + L.offPred );
   int*      sSumA = reinterpret_cast<int*>( smemRaw + L.offSumA );
@@ -174,7 +200,7 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
   unsigned char* sMv8 = smemRaw + L.offMv8;
   uint32_t* sMvRaw = reinterpret_cast<uint32_t*>( smemRaw + L.offMvRaw );
   uint32_t* T     = reinterpret_cast<uint32_t*>( smemRaw + L.offT );
-  uint16_t* Hs    = reinterpret_cast<uint16_t*>( smemRaw + L.offT );
+  uint16_t* Hs    = reinterpret_cast<uint16_t*>( smemRaw + L.offWin1 );         // row sums: prologue scratch in win1, which is formed after the box sums
 
 #ifdef VVB_PYR_PHASES
   unsigned long long pyrT = threadIdx.x == 0 ? pyr_now() : 0ull;
@@ -192,6 +218,9 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
     const int k = i / PYR_MVN, b = i - k * PYR_MVN;
     reinterpret_cast<uint32_t*>( sMv8 )[i] = ( b < VVB_MVCOST_ENTRIES ? par.tab.cost[b] : PYR_NEVER ) * 8u + (uint32_t) k;
   }
+  // the 32x32 tables start zeroed; the argmin pass clears every entry it reads, and a root that skips its candidates leaves them untouched, so every root
+  // finds them zeroed (the first barrier of the root loop publishes this)
+  if( LV >= 3 ) { for( int i = tid; i < L.nT * L.tStride; i += nthr ) T[i] = 0u; }
 
   // A 64x64 CTA walks a run of consecutive roots (gridDim.x runs of balanced length); smaller roots take one CTA each.  carry: the window in shared memory is
   // the previous root's, this root lies one root width to its right with the same rows and range, and the staging area holds this root's new R pels of
@@ -200,6 +229,7 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
   const int rBeg = WALK ? rootFirst + (int)( (long long) blockIdx.x * nRoots / gridDim.x ) : rootFirst + (int) blockIdx.x;
   const int rEnd = WALK ? rootFirst + (int)( (long long)( blockIdx.x + 1 ) * nRoots / gridDim.x ) : rBeg + 1;
   bool carry = false;
+  bool orgStaged = false;                 // orgN holds this root's originals, copied behind the previous root's loop
 #pragma unroll 1
   for( int root = rBeg; root < rEnd; root++ )
   {
@@ -229,7 +259,8 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
         vvb_best b; b.dx = 0; b.dy = 0; b.sad = 0xffffffffu; b.cost = ~0ull;
         lv.best[l][( (size_t) root << ( 2 * ( LTOP - l ) ) ) + i] = b;
       }
-      carry = false;                      // this root's staged columns are dropped; the next root restages in full
+      carry = false;                      // this root's staged columns and originals are dropped; the next root restages in full
+      orgStaged = false;
       continue;
     }
 
@@ -267,7 +298,7 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
             v[u] = 0u;
             if( i < total )
             {
-              const int r = div_rcp( i, inv ), c = i - r * wsw;
+              const int r = pyr_div<NXY>( i, wsw, inv ), c = i - r * wsw;
               if( c < validWords ) v[u] = __ldg( reinterpret_cast<const uint32_t*>( src + (ptrdiff_t) r * refPlane.stride ) + c );
             }
           }
@@ -290,7 +321,7 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
             v[u] = 0;
             if( i < total )
             {
-              const int r = div_rcp( i, inv ), c = i - r * ws;
+              const int r = pyr_div<NXY>( i, ws, inv ), c = i - r * ws;
               if( c < validW ) v[u] = __ldg( src + (ptrdiff_t) r * refPlane.stride + c );
             }
           }
@@ -299,11 +330,15 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
         }
       }
       if( tid < 8 ) win0w[winH * wsw + tid] = 0u;                                   // overrun words read by the shifted copy
-      const int16_t* so = orgPlane.origin + (ptrdiff_t) rb.y * orgPlane.stride + rb.x;
-      for( int i = tid; i < R * R; i += nthr )
+      if( WALK && orgStaged ) { int16_t* t = orgS; orgS = orgN; orgN = t; }
+      else
       {
-        const int r = i / R, c = i - r * R;
-        orgS[i] = __ldg( so + (ptrdiff_t) r * orgPlane.stride + c );
+        const int16_t* so = orgPlane.origin + (ptrdiff_t) rb.y * orgPlane.stride + rb.x;
+        for( int i = tid; i < R * R; i += nthr )
+        {
+          const int r = i / R, c = i - r * R;
+          orgS[i] = __ldg( so + (ptrdiff_t) r * orgPlane.stride + c );
+        }
       }
       for( int i = tid; i < NB0 + NQ; i += nthr ) sKey32[i] = 0xffffffffu;
       if( tid < 8 ) sKey64[tid] = ~0ull;
@@ -311,9 +346,8 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
     __syncthreads();
     PYR_MARK( 1 );
 
-    // ---- shifted copy, per-block sum a, row sums Hs[r][c] = sum_{x<8} win[r][c+x], MV bit counts
+    // ---- per-block sum a, row sums Hs[r][c] = sum_{x<8} win[r][c+x], MV bit counts
     {
-      for( int i = tid; i < winH * wsw; i += nthr ) win1w[i] = __funnelshift_r( win0w[i], win0w[i + 1], 16 );
       for( int b = tid; b < NB0; b += nthr )
       {
         const int bx = pyr_compact( b ), by = pyr_compact( b >> 1 );
@@ -329,7 +363,7 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
       const float inv = 1.0f / (float) cStrips;
       for( int t = tid; t < nTasks; t += nthr )
       {
-        const int r = div_rcp( t, inv ), st = t - r * cStrips;
+        const int r = pyr_div<NXY>( t, cStrips, inv ), st = t - r * cStrips;
         const uint32_t* row = win0w + r * wsw + st * 4;
         const uint4 a = *reinterpret_cast<const uint4*>( row ), b = *reinterpret_cast<const uint4*>( row + 4 );
         const uint32_t w[8] = { a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w };
@@ -346,15 +380,24 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
         }
         *reinterpret_cast<uint4*>( Hs + r * L.vPitch + st * 8 ) = make_uint4( o[0], o[1], o[2], o[3] );
       }
-      const float invB = 1.0f / (float) L.bStride;
-      for( int t = tid; t < NBLK * L.bStride; t += nthr )
+      // a thread per (block, 8 entries): nxp and bStride are multiples of 8, so the 8 entries are all column bits or all row bits
+      const int bChunks = L.bStride >> 3;
+      const float invB = 1.0f / (float) bChunks;
+      for( int t = tid; t < NBLK * bChunks; t += nthr )
       {
-        const int bid = div_rcp( t, invB ), e = t - bid * L.bStride;
+        const int bid = pyr_div<NXY>( t, bChunks, invB ), e0 = 8 * ( t - bid * bChunks );
         const int2 pr = sPred[bid];
-        unsigned char v;
-        if( e < nxp ) v = e < nx ? (unsigned char) eg_bits( ( ( rb.left + e ) * ( 1 << par.costScale ) - pr.x ) >> par.imvShift ) : (unsigned char) PYR_PAD_BITS;
-        else          v = (unsigned char)( 4u * eg_bits( ( ( rb.top + ( e - nxp ) ) * ( 1 << par.costScale ) - pr.y ) >> par.imvShift ) );
-        bitsS[t] = v;
+        uint32_t w[2] = { 0u, 0u };
+#pragma unroll
+        for( int k = 0; k < 8; k++ )
+        {
+          const int e = e0 + k;
+          uint32_t v;
+          if( e0 < nxp ) v = e < nx ? eg_bits( ( ( rb.left + e ) * ( 1 << par.costScale ) - pr.x ) >> par.imvShift ) : (uint32_t) PYR_PAD_BITS;
+          else           v = 4u * eg_bits( ( ( rb.top + ( e - nxp ) ) * ( 1 << par.costScale ) - pr.y ) >> par.imvShift );
+          w[k >> 2] |= ( v & 0xffu ) << ( 8 * ( k & 3 ) );
+        }
+        *reinterpret_cast<uint2*>( bitsS + bid * L.bStride + e0 ) = make_uint2( w[0], w[1] );
       }
     }
     __syncthreads();
@@ -375,13 +418,15 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
       }
     }
     __syncthreads();
-    if( LV >= 3 ) { for( int i = tid; i < L.nT * L.tStride; i += nthr ) T[i] = 0u; }
+    // ---- one-pel-shifted copy of the window, over the row sums
+    for( int i = tid; i < winH * wsw; i += nthr ) win1w[i] = __funnelshift_r( win0w[i], win0w[i + 1], 16 );
     __syncthreads();
     PYR_MARK( 2 );
 
-    // ---- next root of the run: L2 prefetches of its descriptors and originals, and, when it can carry this window, cp.async copies of its new window columns
-    // into the staging area.  They complete behind this root's candidate loop; the wait comes after the results, the next root's first barrier publishes them.
-    bool carryNext = false;
+    // ---- next root of the run: L2 prefetches of its descriptors, cp.async copies of its originals into the other originals buffer (L2 prefetches where the
+    // buffer does not fit or the rows are not 16-byte aligned), and, when it can carry this window, cp.async copies of its new window columns into the staging
+    // area.  They complete behind this root's candidate loop; the wait comes after the results, the next root's first barrier publishes them.
+    bool carryNext = false, orgNext = false;
     if( WALK && root + 1 < rEnd )
     {
       const vvb_block nb = lv.blocks[LTOP][root + 1];
@@ -392,7 +437,16 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
         pyr_prefetch_l2( &lv.blocks[l][( (size_t)( root + 1 ) << ( 2 * ( LTOP - l ) ) ) + i] );
       }
       const int16_t* so = orgPlane.origin + (ptrdiff_t) nb.y * orgPlane.stride + nb.x;
-      if( tid < 2 * R ) pyr_prefetch_l2( so + (ptrdiff_t)( tid >> 1 ) * orgPlane.stride + ( tid & 1 ) * ( R - 1 ) );     // first and last pel of every row
+      orgNext = L.offOrgNext > 0 && ( ( (uintptr_t) so & 15 ) == 0 ) && ( ( orgPlane.stride & 7 ) == 0 );
+      if( orgNext )
+      {
+        for( int i = tid; i < R * ( R / 8 ); i += nthr )
+        {
+          const int r = i / ( R / 8 ), c = i - r * ( R / 8 );
+          pyr_cp_async16( orgN + r * R + 8 * c, so + (ptrdiff_t) r * orgPlane.stride + 8 * c );
+        }
+      }
+      else if( tid < 2 * R ) pyr_prefetch_l2( so + (ptrdiff_t)( tid >> 1 ) * orgPlane.stride + ( tid & 1 ) * ( R - 1 ) );     // first and last pel of every row
       carryNext = L.stageWords > 0 && src32 && nb.x == rb.x + R && nb.y == rb.y && nb.left == rb.left && nb.right == rb.right && nb.top == rb.top &&
                   nb.bottom == rb.bottom;
       if( carryNext )
@@ -442,8 +496,12 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
         {
           const unsigned mask = maskS;
           int q, pr, st;
-          if( it < itemsMain ) { q = div_rcp( it, invPerQm ); const int rem = it - q * perQm; pr = div_rcp( rem, invMain ); st = rem - pr * nMain; }
-          else { const int i2 = it - itemsMain; q = div_rcp( i2, invPerQt ); const int rem = i2 - q * perQt; const int ts = div_rcp( rem, invPairs ); pr = rem - ts * nPairs; st = nMain + ts; }
+          if( it < itemsMain ) { q = pyr_div<NXY>( it, max( 1, perQm ), invPerQm ); const int rem = it - q * perQm; pr = pyr_div<NXY>( rem, max( 1, nMain ), invMain ); st = rem - pr * nMain; }
+          else
+          {
+            const int i2 = it - itemsMain; q = pyr_div<NXY>( i2, max( 1, perQt ), invPerQt ); const int rem = i2 - q * perQt;
+            const int ts = pyr_div<NXY>( rem, nPairs, invPairs ); pr = rem - ts * nPairs; st = nMain + ts;
+          }
           const int cy = 2 * pr, cx0 = 8 * st;
           const bool validB = cy + 1 < ny;
           const int lead = __ffs( mask ) - 1;
@@ -559,8 +617,8 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
           // 15 window rows its 8 vectors touch: window row r meets original row r - c for vector c.
           const unsigned mask = maskC;
           const int ic = it - itemsStrip;
-          const int q = div_rcp( ic, invPerQc ), rem = ic - q * perQc;
-          const int ci = div_rcp( rem, invNv ), g = rem - ci * nV;
+          const int q = pyr_div<NXY>( ic, max( 1, perQc ), invPerQc ), rem = ic - q * perQc;
+          const int ci = pyr_div<NXY>( rem, nV, invNv ), g = rem - ci * nV;
           const int cx = 8 * nFull + ci, cy0 = 8 * g;
           const int lead = __ffs( mask ) - 1;
           const bool uni = __all_sync( mask, q == __shfl_sync( mask, q, lead ) );
@@ -658,14 +716,14 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
       for( int j = 0; j < NTOP; j++ ) best[j] = ~0ull;
       for( int o = tid; o < nx * ny; o += nthr )
       {
-        const int cy = div_rcp( o, invNx ), cx = o - cy * nx;
+        const int cy = pyr_div<NXY>( o, nx, invNx ), cx = o - cy * nx;
         const int ti = cy * nxp + ( cx & 7 ) * nStrips + ( cx >> 3 );
         uint32_t sum = 0u;
 #pragma unroll
         for( int j = 0; j < NTOP; j++ )
         {
           uint32_t s;
-          if( j < NT ) { s = T[j * L.tStride + ti]; sum += s; }
+          if( j < NT ) { s = T[j * L.tStride + ti]; T[j * L.tStride + ti] = 0u; sum += s; }      // cleared for the next root
           else         s = sum;
           const unsigned char* bb = bitsS + ( j < NT ? OFF2 + j : OFF3 ) * L.bStride;
           const uint32_t bits = (uint32_t) bb[cx] + ( (uint32_t) bb[nxp + cy] >> 2 );
@@ -700,8 +758,9 @@ __global__ void __launch_bounds__( pyr_max_threads<LV>(), 1 ) sad_pyramid8_kerne
       b.sad = (uint32_t)( cost - sMvRaw[bits < VVB_MVCOST_ENTRIES ? bits : VVB_MVCOST_ENTRIES - 1] );
       lv.best[l][( (size_t) root << ( 2 * ( LTOP - l ) ) ) + i] = b;
     }
-    if( carryNext ) pyr_cp_async_wait_all();
+    if( carryNext || orgNext ) pyr_cp_async_wait_all();
     carry = carryNext;
+    orgStaged = orgNext;
 #ifdef VVB_PYR_PHASES
     __syncthreads();
     PYR_MARK( 5 );
