@@ -482,6 +482,37 @@ int vvb_mctf_search_grid_dev( vvb_ctx* ctx, int org_plane, int ref_plane, const 
 int vvb_frac_cost_grid    ( vvb_ctx* ctx, int dfunc, int org_plane, int ref_plane, const vvb_block* blocks, int n, int w, int h, int reduce_tap, int alt_hpel, uint32_t* cost_out );
 int vvb_frac_cost_grid_dev( vvb_ctx* ctx, int dfunc, int org_plane, int ref_plane, const vvb_block* dev_blocks, int n, int w, int h, int reduce_tap, int alt_hpel, uint32_t* dev_cost_out );
 
+/* Fractional motion refinement on the device = InterSearch::xPatternSearchFracDIF (EncoderLib/InterSearch.cpp:2678-2724) for every PU of a call, one PU shape per call
+ * (w, h in 4..128, powers of two, not 4x4): the half-pel round and the quarter-pel round of xPatternRefinement (:760-972) with their selection on the device, so the
+ * results equal the member's bit for bit -- the strict `<` in the order of s_acMvRefineH / s_acMvRefineQ, the uiDistBest each round starts from (:769) and the distH
+ * values, and with fast_sub_pel = 1 the early stops (:808-811), the pattern id in wrapping Distortion arithmetic (:886-969) and the s_skipQpelPosition masks; pattern 0
+ * ends the search after the half-pel round (qter stays 0, 0).  The filtered blocks and the distortion are those of vvb_frac_cost_grid.  MV rate: Distortion( sqrt(lambda)
+ * * bits ) as for vvb_tz_search, cost scale 1 in the half-pel round and 0 in the quarter-pel round, imvShift 0 (:2696, :2714, :873).
+ * Inputs are the arrays of vvb_tz_search: pus[i] gives the position (x, y) and the quarter-pel predictor (pred_hor, pred_ver; the other fields are ignored), int_mv[i]
+ * the integer vector (mv_hor, mv_ver; the other fields are ignored), so vvb_tz_search_dev followed by vvb_frac_search_dev chains without a copy.
+ * Reads are not clamped: a PU reads reference columns x + mv_hor - 5 .. x + mv_hor + w + 4 and rows y + mv_ver - 4 .. y + mv_ver + h + 3 (the +-1 pel of the
+ * refinement, the 8-tap reach, and one column on each side for the pel-pair alignment of the window load).  Every vector vvb_tz_search can return is covered by a
+ * reference margin of tz->ctu_size + 12 pels.
+ * Errors: null pointers, negative n, fast_sub_pel outside 0..1 (m_fastSubPel = 2 never calls the member, :2113), reduce_tap outside 0..2, a negative or non-finite lambda,
+ * and (host-buffer call) a PU outside the original plane: VVB_ERR_ARG; shapes outside the domain, a dfunc other than SAD / HAD / HAD_FAST, planes above 12 bits and
+ * (host-buffer call) a PU whose read box leaves the reference margin: VVB_ERR_UNSUPPORTED.  n == 0 returns VVB_OK without a launch.
+ * The _dev twin checks the position and the read box per PU on the device before any read: a PU that fails gets cost = UINT64_MAX and offsets 0 (a real result is
+ * never that value: the half-pel round always evaluates its position 0). */
+typedef struct
+{
+  double  lambda;                  /* RdCost::setLambda                                                                                    */
+  int32_t dfunc;                   /* VVB_DF_SAD / VVB_DF_HAD / VVB_DF_HAD_FAST: m_bUseHADME ? ( m_fastHad ? 2 : 1 ) : 0 (:775)               */
+  int32_t reduce_tap;              /* m_meReduceTap, 0..2                                                                                  */
+  int32_t alt_hpel;                /* cStruct.useAltHpelIf; implies imvShift == IMV_HPEL, i.e. no quarter-pel round (:2711)                */
+  int32_t fast_sub_pel;            /* m_fastSubPel, 0 or 1                                                                                 */
+} vvb_frac_par;
+/* rcMvHalf, rcMvQter (offsets in half / quarter pel) and ruiCost as the member returns them */
+typedef struct { int16_t half_hor, half_ver, qter_hor, qter_ver; uint64_t cost; } vvb_frac_best;   /* 16 bytes */
+int vvb_frac_search    ( vvb_ctx* ctx, int org_plane, int ref_plane, const vvb_tz_pu* pus, const vvb_tz_best* int_mv, int n, int w, int h,
+                         const vvb_frac_par* par, vvb_frac_best* out );
+int vvb_frac_search_dev( vvb_ctx* ctx, int org_plane, int ref_plane, const vvb_tz_pu* dev_pus, const vvb_tz_best* dev_int_mv, int n, int w, int h,
+                         const vvb_frac_par* par, vvb_frac_best* dev_out );
+
 /* ---- MCTF apply stage (SURVEY 8f-3): the per-block body of MCTF::xFinalizeBlkLine (MCTF.cpp:1437-1483) for the luma plane, fused:
  * per reference picture applyFrac (m_applyFrac, :259-357) at the block's vector, applyPlanarCorrection (:372-420) when rmsme > 0 and
  * planar_correction (the caller passes m_QP <= 32) and the block is square <= 32, then applyBlock (:422-518: noise estimate, weights, bilateral

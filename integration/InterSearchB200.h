@@ -112,10 +112,10 @@ inline void xPatternSearchB200( InterSearch& is, InterSearch::TZSearchStruct& cS
 // xPatternRefinement filters itself, :812-848) and every distortion call of xPatternRefinement come back as ONE 7x7 table t[j+3][i+3] (quarter-pel offset (i, j)
 // from rcMvInt; vvb_frac_cost_grid: SAD, SATD or fast SATD, square and rectangular PUs); the two rounds are replayed on it.
 //   m_fastSubPel == 0 (slower): both rounds visit all nine positions, each round starts from MAX_DISTORTION.
-//   m_fastSubPel == 1 (fast ... slow): the half-pel round stops early (:808-811) and classifies the cost surface into a pattern id (:886-969); the quarter-pel round
+//   m_fastSubPel == 1 (faster ... slow): the half-pel round stops early (:808-811) and classifies the cost surface into a pattern id (:886-969); the quarter-pel round
 //     visits only what s_skipQpelPosition allows for that pattern (:93-137 -- file-static in the reference, restated here as one 9-bit mask per pattern, bit i =
 //     position i skipped) and keeps the half-pel best as its threshold (:769); pattern 0 ends the search after the half-pel round (:2710) with rcMvQter untouched.
-//   m_fastSubPel == 2 (faster): xMotionEstimation does not call the function (:2113).
+//   m_fastSubPel == 2 (the first pass of a two-pass encode, vvencCfg.cpp:2661): xMotionEstimation does not call the function (:2113).
 inline void xPatternSearchFracDIFB200( InterSearch& is, InterSearch::TZSearchStruct& cStruct, const Mv& rcMvInt, Mv& rcMvHalf, Mv& rcMvQter, Distortion& ruiCost )
 {
   const VVEncCfg& cfg = *is.m_pcEncCfg;

@@ -30,6 +30,13 @@ class vvb_tz_par(ctypes.Structure):
     _fields_ = [(k, ctypes.c_int32) for k in ('search_range', 'extended', 'fast', 'integer_et', 'first_search_stop', 'sub_shift_mode', 'pic_w', 'pic_h', 'ctu_size', 'ifp_lines')]
 
 
+class vvb_frac_par(ctypes.Structure):
+    _fields_ = [('lam', ctypes.c_double), ('dfunc', ctypes.c_int32), ('reduce_tap', ctypes.c_int32), ('alt_hpel', ctypes.c_int32), ('fast_sub_pel', ctypes.c_int32)]
+
+
+FRAC_PAR = vvb_frac_par
+
+
 class vvb_tu_par(ctypes.Structure):
     _fields_ = [('w', ctypes.c_int32), ('h', ctypes.c_int32), ('tr_hor', ctypes.c_int32), ('tr_ver', ctypes.c_int32), ('bit_depth', ctypes.c_int32),
                 ('qp', ctypes.c_int32), ('is_irap', ctypes.c_int32), ('dep_quant', ctypes.c_int32), ('sign_hiding', ctypes.c_int32), ('lfnst_idx', ctypes.c_int32), ('lfnst_set', ctypes.c_int32), ('lfnst_transpose', ctypes.c_int32),
@@ -95,6 +102,8 @@ MCTF_DT = np.dtype([('x', '<i4'), ('y', '<i4'), ('mvx', '<i4'), ('mvy', '<i4'), 
 TZ_PU_DT = np.dtype([('x', '<i4'), ('y', '<i4'), ('start_hor', '<i4'), ('start_ver', '<i4'), ('pred_hor', '<i2'), ('pred_ver', '<i2'), ('cand_first', '<i4'), ('cand_count', '<i4')])
 TZ_BEST_DT = np.dtype([('mv_hor', '<i4'), ('mv_ver', '<i4'), ('sad', '<u8'), ('cost', '<u8'), ('best_distance', '<u4'), ('pad', '<u4')])
 assert TZ_PU_DT.itemsize == 28 and TZ_BEST_DT.itemsize == 32
+FRAC_BEST_DT = np.dtype([('half_hor', '<i2'), ('half_ver', '<i2'), ('qter_hor', '<i2'), ('qter_ver', '<i2'), ('cost', '<u8')])
+assert FRAC_BEST_DT.itemsize == 16 and ctypes.sizeof(vvb_frac_par) == 24
 assert CAND_DT.itemsize == 32 and BLOCK_DT.itemsize == 24 and BEST_DT.itemsize == 16 and MCTF_DT.itemsize == 20
 
 # every symbol include/vvenc_b200.h declares: name -> (restype, argtypes)
@@ -178,6 +187,8 @@ SYMBOLS = {
     'vvb_mctf_search_grid_dev': (c_i, [c_p, c_i, c_i, c_p, c_i, c_i, c_i, c_i, c_p]),
     'vvb_frac_cost_grid': (c_i, [c_p, c_i, c_i, c_i, c_p, c_i, c_i, c_i, c_i, c_i, c_p]),
     'vvb_frac_cost_grid_dev': (c_i, [c_p, c_i, c_i, c_i, c_p, c_i, c_i, c_i, c_i, c_i, c_p]),
+    'vvb_frac_search': (c_i, [c_p, c_i, c_i, c_p, c_p, c_i, c_i, c_i, ctypes.POINTER(vvb_frac_par), c_p]),
+    'vvb_frac_search_dev': (c_i, [c_p, c_i, c_i, c_p, c_p, c_i, c_i, c_i, ctypes.POINTER(vvb_frac_par), c_p]),
     'vvb_mctf_apply': (c_i, [c_p, c_i, ctypes.POINTER(vvb_mctf_apply_par), c_p, c_p, c_i]),
     'vvb_mctf_apply_dev': (c_i, [c_p, c_i, ctypes.POINTER(vvb_mctf_apply_par), c_p, c_p, c_i]),
     'vvb_mctf_calc_var': (c_i, [c_p, c_i, c_p, c_i, c_p]),

@@ -5,7 +5,7 @@
 
   getDistPart-like single calls .... dist_block / sad_mask_block / sad_x5_block / fix_wsse_block   (RdCost.h:74-75,117)
   batched candidate evaluation ..... dist_batch (descriptor list), dist_pool (RDO candidate pools)
-  motion search .................... sad_search (xPatternSearch), sad_pattern (fixed TZ point set), tz_search (xTZSearch walk)
+  motion search .................... sad_search (xPatternSearch), sad_pattern (fixed TZ point set), tz_search (xTZSearch walk), frac_search (xPatternSearchFracDIF)
   TU coding ........................ fwd_trquant (TrQuant::transformNxN: xT + Quant::quant + xNeedRDOQ)
   pre-analysis ..................... mctf_error_batch (MCTF::motionErrorLuma)
   affine ME ........................ affine_sobel / affine_equal_coeff
@@ -269,6 +269,20 @@ class CostEngine:
         blocks = np.ascontiguousarray(blocks, dtype=L.BLOCK_DT)
         out = np.zeros((len(blocks), 7, 7), dtype=np.uint32)
         self._chk(self.lib.vvb_frac_cost_grid(self.h, dfunc, org_plane, ref_plane, _p(blocks), len(blocks), w, h, int(reduce_tap), int(alt_hpel), _p(out)))
+        return out
+
+    @staticmethod
+    def frac_par(lambda_, dfunc, reduce_tap=2, alt_hpel=False, fast_sub_pel=1):
+        return L.vvb_frac_par(float(lambda_), dfunc, reduce_tap, int(alt_hpel), fast_sub_pel)
+
+    def frac_search(self, org_plane, ref_plane, pus, int_mv, w, h, par):
+        """InterSearch::xPatternSearchFracDIF for every PU of one shape.  pus: TZ_PU_DT array (x, y, pred_hor, pred_ver used); int_mv: TZ_BEST_DT array
+        (mv_hor, mv_ver used), e.g. what tz_search returned.  Returns a FRAC_BEST_DT array (rcMvHalf, rcMvQter, ruiCost)."""
+        pus = np.ascontiguousarray(pus, dtype=L.TZ_PU_DT)
+        int_mv = np.ascontiguousarray(int_mv, dtype=L.TZ_BEST_DT)
+        assert len(pus) == len(int_mv)
+        out = np.zeros(len(pus), dtype=L.FRAC_BEST_DT)
+        self._chk(self.lib.vvb_frac_search(self.h, org_plane, ref_plane, _p(pus), _p(int_mv), len(pus), w, h, ctypes.byref(par), _p(out)))
         return out
 
     # ---- dependent quantisation

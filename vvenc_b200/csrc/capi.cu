@@ -22,6 +22,7 @@
 #include "batch_kernels.cuh"
 #include "mctf_control_kernels.cuh"
 #include "tz_kernels.cuh"
+#include "frac_search_kernels.cuh"
 #include "depquant_host.h"
 #include "rdoq_host.h"
 #include "vvc_tables.h"
@@ -423,7 +424,7 @@ int vvb_create( vvb_ctx** out, int device )
     VVB_RING_SMEM( 16 ), VVB_RING_SMEM( 32 ), VVB_RING_SMEM( 64 ),
     smemLimit( mctf_error_packed_kernel, 100 * 1024 ), smemLimit( mctf_grid_kernel, 200 * 1024 ), smemLimit( mctf_wave_kernel, 100 * 1024 ),
     smemLimit( mctf_int_grid_kernel, 100 * 1024 ), smemLimit( mctf_apply_kernel, 100 * 1024 ), smemLimit( frac_grid_kernel, 100 * 1024 ),
-    smemLimit( frac_grid_generic_kernel, 100 * 1024 ),
+    smemLimit( frac_grid_generic_kernel, 100 * 1024 ), smemLimit( frac_search_kernel, FRAC_SEARCH_SMEM ),
     VVB_FWD_TC_SMEM( 8 ), VVB_FWD_TC_SMEM( 16 ), VVB_FWD_TC_SMEM( 32 ), VVB_FWD_TC_SMEM( 64 ), VVB_ITC_SMEM( 8 ), VVB_ITC_SMEM( 16 ), VVB_ITC_SMEM( 32 ), VVB_ITC_SMEM( 64 ) };
 #undef VVB_FWD_TC_SMEM
 #undef VVB_ITC_SMEM
@@ -2245,6 +2246,66 @@ int vvb_frac_cost_grid( vvb_ctx* ctx, int dfunc, int orgPlane, int refPlane, con
   const vvb_block* dB; uint32_t* dC;
   return HostCall( ctx ).in( dB, blocks, n ).out( dC, cost, (size_t) n * 49 )
                         .run( [&] { return vvb_frac_cost_grid_dev( ctx, dfunc, orgPlane, refPlane, dB, n, w, h, reduceTap, altHpel, dC ); } );
+}
+
+// ---- fractional refinement with the selection on the device (xPatternSearchFracDIF) --------------------------------------------------------
+static int fracSearchSetup( vvb_ctx* ctx, int orgPlane, int refPlane, int n, int w, int h, const vvb_frac_par* par, FracSearchPar& fp, FracFilter& flt, MePar& mpHalf, MePar& mpQter )
+{
+  if( !par || n < 0 ) return fail( ctx, VVB_ERR_ARG, "bad arguments" );
+  if( !validPlane( ctx, orgPlane ) || !validPlane( ctx, refPlane ) ) return fail( ctx, VVB_ERR_ARG, "unknown plane" );
+  if( par->fast_sub_pel != 0 && par->fast_sub_pel != 1 ) return fail( ctx, VVB_ERR_ARG, "fast_sub_pel is 0 or 1 (m_fastSubPel = 2 has no fractional search, InterSearch.cpp:2113)" );
+  if( par->reduce_tap < 0 || par->reduce_tap > 2 ) return fail( ctx, VVB_ERR_ARG, "reduce_tap is 0, 1 or 2" );
+  if( !std::isfinite( par->lambda ) || par->lambda < 0 ) return fail( ctx, VVB_ERR_ARG, "lambda must be finite and not negative" );
+  if( par->dfunc != VVB_DF_SAD && par->dfunc != VVB_DF_HAD && par->dfunc != VVB_DF_HAD_FAST ) return fail( ctx, VVB_ERR_UNSUPPORTED, "fractional search: SAD, HAD or HAD_fast" );
+  // 4x4 is not an inter PU (the member would switch to its 4x4 filter there)
+  if( !isPow2( w ) || !isPow2( h ) || w < 4 || h < 4 || w > 128 || h > 128 || w * h == 16 ) return fail( ctx, VVB_ERR_UNSUPPORTED, "fractional search: PU sides 4..128, powers of two, not 4x4" );
+  if( ctx->planes.p[orgPlane].bitDepth > 12 || ctx->planes.p[refPlane].bitDepth > 12 ) return fail( ctx, VVB_ERR_UNSUPPORTED, "fractional search: planes of up to 12 bits" );
+  const vvb_me_par me{ par->lambda, 1, 0, 0, 0, 0, 0 };                    // cost scale 1 (half pel, :2696), imvShift 0
+  int rc = makeMePar( ctx, &me, mpHalf );
+  if( rc ) return rc;
+  mpQter = mpHalf; mpQter.costScale = 0;                                    // quarter pel (:2714)
+  flt = frac_filter( par->reduce_tap, par->alt_hpel != 0 );
+  const FracSearchSmem L = frac_search_smem( w, h );
+  fp.w = w; fp.h = h; fp.family = par->dfunc == VVB_DF_SAD ? 1 : par->dfunc == VVB_DF_HAD ? 2 : 3;
+  fp.fast = par->fast_sub_pel; fp.quarter = par->alt_hpel == 0;
+  fp.slots = std::min( 9, ( FRAC_SEARCH_SMEM / 4 - L.base ) / L.slotWords );      // three for 128x128: a group of one horizontal offset
+  return VVB_OK;
+}
+
+int vvb_frac_search_dev( vvb_ctx* ctx, int orgPlane, int refPlane, const vvb_tz_pu* dPus, const vvb_tz_best* dIntMv, int n, int w, int h, const vvb_frac_par* par, vvb_frac_best* dOut )
+{
+  if( !ctx || !dPus || !dIntMv || !dOut ) return fail( ctx, VVB_ERR_ARG, "bad arguments" );
+  FracSearchPar fp; FracFilter flt; MePar mpHalf, mpQter;
+  int rc = fracSearchSetup( ctx, orgPlane, refPlane, n, w, h, par, fp, flt, mpHalf, mpQter );
+  if( rc || n == 0 ) return rc;
+  CU( cudaSetDevice( ctx->device ) );
+  const FracSearchSmem L = frac_search_smem( w, h );
+  const size_t smem = (size_t)( L.base + fp.slots * L.slotWords ) * 4;
+  const int threads = w * h >= 64 * 64 ? 256 : 128;
+  int perSm = 0;
+  CU( cudaOccupancyMaxActiveBlocksPerMultiprocessor( &perSm, frac_search_kernel, threads, smem ) );
+  const int grid = (int) std::min<long long>( n, (long long) ctx->numSMs * std::max( 1, perSm ) );
+  frac_search_kernel<<<grid, threads, smem, ctx->stream>>>( ctx->planes.p[orgPlane], ctx->planes.p[refPlane], dPus, dIntMv, n, fp, flt, mpHalf, mpQter, dOut );
+  CHECK_LAUNCH( "frac_search_kernel" );
+  return VVB_OK;
+}
+
+int vvb_frac_search( vvb_ctx* ctx, int orgPlane, int refPlane, const vvb_tz_pu* pus, const vvb_tz_best* intMv, int n, int w, int h, const vvb_frac_par* par, vvb_frac_best* out )
+{
+  if( !ctx || !pus || !intMv || !out ) return fail( ctx, VVB_ERR_ARG, "bad arguments" );
+  FracSearchPar fp; FracFilter flt; MePar mpHalf, mpQter;
+  int rc = fracSearchSetup( ctx, orgPlane, refPlane, n, w, h, par, fp, flt, mpHalf, mpQter );
+  if( rc || n == 0 ) return rc;
+  const Plane &op = ctx->planes.p[orgPlane], &rp = ctx->planes.p[refPlane];
+  for( int i = 0; i < n; i++ )
+  {
+    if( pus[i].x < 0 || pus[i].y < 0 || pus[i].x > op.width - w || pus[i].y > op.height - h ) return fail( ctx, VVB_ERR_ARG, "PU outside the original plane" );
+    if( !frac_search_admitted( rp, pus[i].x, pus[i].y, intMv[i].mv_hor, intMv[i].mv_ver, w, h ) )
+      return fail( ctx, VVB_ERR_UNSUPPORTED, "read box outside the reference margin (columns x + mv - 5 .. x + mv + w + 4, rows y + mv - 4 .. y + mv + h + 3)" );
+  }
+  const vvb_tz_pu* dP; const vvb_tz_best* dM; vvb_frac_best* dO;
+  return HostCall( ctx ).in( dP, pus, n ).in( dM, intMv, n ).out( dO, out, n )
+                        .run( [&] { return vvb_frac_search_dev( ctx, orgPlane, refPlane, dP, dM, n, w, h, par, dO ); } );
 }
 
 // ---- MCTF apply stage (xFinalizeBlkLine body per block) ---------------------------------------------------------------------
