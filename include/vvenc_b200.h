@@ -513,6 +513,74 @@ int vvb_frac_search    ( vvb_ctx* ctx, int org_plane, int ref_plane, const vvb_t
 int vvb_frac_search_dev( vvb_ctx* ctx, int org_plane, int ref_plane, const vvb_tz_pu* dev_pus, const vvb_tz_best* dev_int_mv, int n, int w, int h,
                          const vvb_frac_par* par, vvb_frac_best* dev_out );
 
+/* Bi-predictive motion refinement on the device = the bBi branch of InterSearch::xMotionEstimation (EncoderLib/InterSearch.cpp:1976-2132) with cu.imv IMV_OFF or
+ * IMV_HPEL, for every PU of a call, one PU shape per call (w, h in 4..128, powers of two, no larger than par->ctu_size, not 4x4 / 4x8 / 8x4: CU::isBipredRestriction).
+ *   target   the search key is 2 * org - pred (AreaBuf::removeHighFreq, Buffer.h:448-480), ClipPel( 2 * org - pred ) with par->clip; pred is the other list's
+ *            prediction, passed per PU as a compact w x h block of pred[n][h][w] in the original's bit depth.  The target spans -(2^bd - 1) .. 2^(bd + 1) - 2 and is
+ *            held as int16 (bd <= 12); the distortion takes it in signed arithmetic, no packed format that assumes samples in 0 .. 2^bd - 1.
+ *   start    (:2051-2090) the SAD + MV rate of the start vector (start_hor / ver, xClipMvSearch with ifp_lines, then changePrecision to integer pel), then of every
+ *            candidate cands[cand_first .. +cand_count) that does not repeat an earlier one of the list, clipped the same way; strict `<`; the window is centred
+ *            on the unclipped winner.
+ *   integer  xSetSearchRange( bestInitMv, search_range ) and xPatternSearch (:2209-2251): SAD over the window in raster order, first strictly smaller cost wins; MV
+ *            rate at cost scale 2 and imvShift (1 with IMV_HPEL); row sub-sampling from sub_shift_mode as RdCost::setDistParam (RdCost.cpp:185-200).  The full SAD
+ *            is always summed: the member's early exit is decision-equivalent.
+ *   fraction xPatternSearchFracDIF (:2678-2724) on the target, exactly as vvb_frac_search (dfunc, reduce_tap, fast_sub_pel; IMV_HPEL: the alternative half-pel
+ *            filter and no quarter-pel round).  fast_sub_pel == 2 has no fractional stage: frac_cost is xPatternSearch's ruiSAD (the SAD without the rate).
+ *   final    (:2117-2124) rcMv = ( int << 2 ) + ( half << 1 ) + qter in quarter pel; uiMvBits at cost scale 0 and imvShift; bits = ruiBits + uiMvBits (uint32);
+ *            cost = (Distortion)( floor( fWeight * ( (double) frac_cost - (double) getCost( uiMvBits ) ) ) + (double) getCost( bits ) ) in IEEE double without
+ *            contraction, getCost( b ) = Distortion( sqrt( lambda ) * b ), fWeight = | getBcwWeight( bcw_idx, ref_list ) | / 8 ({ -2, 3, 4, 5, 10 }, Rom.cpp:1152-1163)
+ *            or 0.5 for bcw_idx 2 (BCW_DEFAULT).  The (Distortion) conversion is the x86-64 one the encoder is built with (cvttsd2si below 2^63, cvttsd2si of
+ *            v - 2^63 with the top bit flipped at or above; cvttsd2si yields 2^63 outside the int64 range): a negative value -k becomes 2^64 - k, as happens with
+ *            fast_sub_pel == 2, a SAD of 0, weight 1.25 and few bits; a value at or above 2^64 becomes 0, as happens with fast_sub_pel == 2 and weight 1.25 when the
+ *            search window is empty (xPatternSearch's cost is then MAX_DISTORTION).
+ *            mv = rcMv in internal units (1/16 pel).
+ * Domain: bit depths 8..12; search_range 0..VVB_BIPRED_MAX_RANGE; dfunc SAD with fast_sub_pel 1 only for w < 64 (for wider PUs the member's AVX2 SAD returns
+ * early-exit partial sums, RdCostX86.h:372-405, which xPatternRefinement keeps in distH and turns into its pattern id); imv 1 (IMV_FPEL) and 2 (IMV_4PEL) go to xPatternSearchIntRefine in the encoder and are VVB_ERR_UNSUPPORTED.
+ * Reads are not clamped.  A PU reads the blocks at its clipped start and candidate vectors, the blocks of the window around each of them (the zero vector when a
+ * window is empty) and the fractional stage's box around the winner (columns mv - 5 .. mv + w + 4, rows mv - 4 .. mv + h + 3, as vvb_frac_search).  Every vector
+ * the clip rules allow is covered by a reference margin of ctu_size + 12 pels (beyond the picture's right and bottom edges w + 12 columns and h + 11 rows suffice).
+ * Errors: null pointers, negative counts, settings out of range, a negative or non-finite lambda and (host-buffer call) PUs outside the picture, candidate ranges
+ * outside cands or a bcw_idx outside 0..4: VVB_ERR_ARG; shapes, imv or dfunc / fast_sub_pel outside the domain, planes above 12 bits, an original plane smaller than the picture and
+ * (host-buffer call) a PU whose read box leaves the reference margin: VVB_ERR_UNSUPPORTED.  n == 0 returns VVB_OK without a launch.
+ * The _dev twin checks each PU on the device before any read: a PU that fails gets cost = frac_cost = int_best = UINT64_MAX and zero vectors and bits. */
+#define VVB_BIPRED_MAX_RANGE 8
+typedef struct
+{
+  int32_t x, y;                    /* PU position in the original plane (inside the picture)                                                             */
+  int32_t start_hor, start_ver;    /* rcMv on entry: internal units (1/16 pel), not clipped                                                              */
+  int16_t pred_hor, pred_ver;      /* RdCost::setPredictor, quarter pel (as vvb_tz_pu)                                                                   */
+  int32_t cand_first, cand_count;  /* m_BlkUniMvInfoBuffer's uniMvs[refPicList][iRefIdxPred] as cands[cand_first .. +cand_count), buffer order, internal units */
+  uint32_t bits;                   /* ruiBits on entry                                                                                                   */
+  int32_t bcw_idx;                 /* cu.BcwIdx, 0..4                                                                                                    */
+} vvb_bi_pu;                       /* 36 bytes */
+typedef struct
+{
+  double  lambda;                  /* RdCost::setLambda                                                                                                  */
+  int32_t search_range;            /* m_bipredSearchRange, 0..VVB_BIPRED_MAX_RANGE                                                                      */
+  int32_t sub_shift_mode;          /* TZSearchStruct::subShiftMode, 0..2                                                                                 */
+  int32_t pic_w, pic_h, ctu_size, ifp_lines;   /* pcv.lumaWidth, pcv.lumaHeight, pcv.maxCUSize (16..128), m_pcEncCfg->m_ifpLines                      */
+  int32_t ref_list;                /* refPicList being refined, 0 or 1                                                                                  */
+  int32_t clip;                    /* m_bClipForBiPredMeEnabled                                                                                         */
+  int32_t imv;                     /* cu.imv: 0 IMV_OFF or 3 IMV_HPEL                                                                                    */
+  int32_t fast_sub_pel;            /* m_fastSubPel, 0..2                                                                                                 */
+  int32_t dfunc;                   /* fractional stage: VVB_DF_SAD / VVB_DF_HAD / VVB_DF_HAD_FAST                                                        */
+  int32_t reduce_tap;              /* m_meReduceTap, 0..2                                                                                                */
+} vvb_bi_par;                      /* 56 bytes */
+typedef struct
+{
+  int32_t int_hor, int_ver;        /* xPatternSearch's rcMv, integer pel                                                                                 */
+  uint64_t int_best;               /* cStruct.uiBestSad                                                                                                  */
+  uint64_t frac_cost;              /* ruiCost after xPatternSearchFracDIF (xPatternSearch's ruiSAD with fast_sub_pel == 2)                               */
+  int16_t half_hor, half_ver, qter_hor, qter_ver;   /* rcMvHalf, rcMvQter                                                                            */
+  int32_t mv_hor, mv_ver;          /* final rcMv, internal units                                                                                         */
+  uint32_t bits, pad;              /* final ruiBits                                                                                                      */
+  uint64_t cost;                   /* final ruiCost                                                                                                      */
+} vvb_bi_best;                     /* 56 bytes */
+int vvb_bipred_search    ( vvb_ctx* ctx, int org_plane, int ref_plane, const vvb_bi_pu* pus, int n, int w, int h, const vvb_bi_par* par,
+                           const int32_t* cands /* [n_cands][2]; nullable when n_cands == 0 */, int n_cands, const int16_t* pred /* [n][h][w] */, vvb_bi_best* out );
+int vvb_bipred_search_dev( vvb_ctx* ctx, int org_plane, int ref_plane, const vvb_bi_pu* dev_pus, int n, int w, int h, const vvb_bi_par* par,
+                           const int32_t* dev_cands, int n_cands, const int16_t* dev_pred, vvb_bi_best* dev_out );
+
 /* ---- MCTF apply stage (SURVEY 8f-3): the per-block body of MCTF::xFinalizeBlkLine (MCTF.cpp:1437-1483) for the luma plane, fused:
  * per reference picture applyFrac (m_applyFrac, :259-357) at the block's vector, applyPlanarCorrection (:372-420) when rmsme > 0 and
  * planar_correction (the caller passes m_QP <= 32) and the block is square <= 32, then applyBlock (:422-518: noise estimate, weights, bilateral

@@ -37,6 +37,11 @@ class vvb_frac_par(ctypes.Structure):
 FRAC_PAR = vvb_frac_par
 
 
+class vvb_bi_par(ctypes.Structure):
+    _fields_ = [('lam', ctypes.c_double)] + [(k, ctypes.c_int32) for k in ('search_range', 'sub_shift_mode', 'pic_w', 'pic_h', 'ctu_size', 'ifp_lines', 'ref_list',
+                                                                          'clip', 'imv', 'fast_sub_pel', 'dfunc', 'reduce_tap')]
+
+
 class vvb_tu_par(ctypes.Structure):
     _fields_ = [('w', ctypes.c_int32), ('h', ctypes.c_int32), ('tr_hor', ctypes.c_int32), ('tr_ver', ctypes.c_int32), ('bit_depth', ctypes.c_int32),
                 ('qp', ctypes.c_int32), ('is_irap', ctypes.c_int32), ('dep_quant', ctypes.c_int32), ('sign_hiding', ctypes.c_int32), ('lfnst_idx', ctypes.c_int32), ('lfnst_set', ctypes.c_int32), ('lfnst_transpose', ctypes.c_int32),
@@ -104,6 +109,12 @@ TZ_BEST_DT = np.dtype([('mv_hor', '<i4'), ('mv_ver', '<i4'), ('sad', '<u8'), ('c
 assert TZ_PU_DT.itemsize == 28 and TZ_BEST_DT.itemsize == 32
 FRAC_BEST_DT = np.dtype([('half_hor', '<i2'), ('half_ver', '<i2'), ('qter_hor', '<i2'), ('qter_ver', '<i2'), ('cost', '<u8')])
 assert FRAC_BEST_DT.itemsize == 16 and ctypes.sizeof(vvb_frac_par) == 24
+BI_PU_DT = np.dtype([('x', '<i4'), ('y', '<i4'), ('start_hor', '<i4'), ('start_ver', '<i4'), ('pred_hor', '<i2'), ('pred_ver', '<i2'), ('cand_first', '<i4'), ('cand_count', '<i4'),
+                     ('bits', '<u4'), ('bcw_idx', '<i4')])
+BI_BEST_DT = np.dtype([('int_hor', '<i4'), ('int_ver', '<i4'), ('int_best', '<u8'), ('frac_cost', '<u8'), ('half_hor', '<i2'), ('half_ver', '<i2'), ('qter_hor', '<i2'),
+                       ('qter_ver', '<i2'), ('mv_hor', '<i4'), ('mv_ver', '<i4'), ('bits', '<u4'), ('pad', '<u4'), ('cost', '<u8')])
+BI_PAR = vvb_bi_par
+assert BI_PU_DT.itemsize == 36 and BI_BEST_DT.itemsize == 56 and ctypes.sizeof(vvb_bi_par) == 56
 assert CAND_DT.itemsize == 32 and BLOCK_DT.itemsize == 24 and BEST_DT.itemsize == 16 and MCTF_DT.itemsize == 20
 
 # every symbol include/vvenc_b200.h declares: name -> (restype, argtypes)
@@ -189,6 +200,8 @@ SYMBOLS = {
     'vvb_frac_cost_grid_dev': (c_i, [c_p, c_i, c_i, c_i, c_p, c_i, c_i, c_i, c_i, c_i, c_p]),
     'vvb_frac_search': (c_i, [c_p, c_i, c_i, c_p, c_p, c_i, c_i, c_i, ctypes.POINTER(vvb_frac_par), c_p]),
     'vvb_frac_search_dev': (c_i, [c_p, c_i, c_i, c_p, c_p, c_i, c_i, c_i, ctypes.POINTER(vvb_frac_par), c_p]),
+    'vvb_bipred_search': (c_i, [c_p, c_i, c_i, c_p, c_i, c_i, c_i, ctypes.POINTER(vvb_bi_par), c_p, c_i, c_p, c_p]),
+    'vvb_bipred_search_dev': (c_i, [c_p, c_i, c_i, c_p, c_i, c_i, c_i, ctypes.POINTER(vvb_bi_par), c_p, c_i, c_p, c_p]),
     'vvb_mctf_apply': (c_i, [c_p, c_i, ctypes.POINTER(vvb_mctf_apply_par), c_p, c_p, c_i]),
     'vvb_mctf_apply_dev': (c_i, [c_p, c_i, ctypes.POINTER(vvb_mctf_apply_par), c_p, c_p, c_i]),
     'vvb_mctf_calc_var': (c_i, [c_p, c_i, c_p, c_i, c_p]),

@@ -5,7 +5,8 @@
 
   getDistPart-like single calls .... dist_block / sad_mask_block / sad_x5_block / fix_wsse_block   (RdCost.h:74-75,117)
   batched candidate evaluation ..... dist_batch (descriptor list), dist_pool (RDO candidate pools)
-  motion search .................... sad_search (xPatternSearch), sad_pattern (fixed TZ point set), tz_search (xTZSearch walk), frac_search (xPatternSearchFracDIF)
+  motion search .................... sad_search (xPatternSearch), sad_pattern (fixed TZ point set), tz_search (xTZSearch walk), frac_search (xPatternSearchFracDIF),
+                                     bipred_search (the bi-predictive branch of xMotionEstimation)
   TU coding ........................ fwd_trquant (TrQuant::transformNxN: xT + Quant::quant + xNeedRDOQ)
   pre-analysis ..................... mctf_error_batch (MCTF::motionErrorLuma)
   affine ME ........................ affine_sobel / affine_equal_coeff
@@ -283,6 +284,23 @@ class CostEngine:
         assert len(pus) == len(int_mv)
         out = np.zeros(len(pus), dtype=L.FRAC_BEST_DT)
         self._chk(self.lib.vvb_frac_search(self.h, org_plane, ref_plane, _p(pus), _p(int_mv), len(pus), w, h, ctypes.byref(par), _p(out)))
+        return out
+
+    @staticmethod
+    def bi_par(lambda_, search_range, pic_w, pic_h, ctu_size, dfunc, ref_list=0, clip=False, imv=0, fast_sub_pel=1, reduce_tap=2, sub_shift_mode=1, ifp_lines=0):
+        return L.vvb_bi_par(float(lambda_), search_range, sub_shift_mode, pic_w, pic_h, ctu_size, ifp_lines, ref_list, int(clip), imv, fast_sub_pel, dfunc, reduce_tap)
+
+    def bipred_search(self, org_plane, ref_plane, pus, w, h, par, pred, cands=None):
+        """The bi-predictive branch of InterSearch::xMotionEstimation for every PU of one shape.  pus: BI_PU_DT array; pred: int16 [n][h][w], the other list's
+        prediction per PU; cands: int32 [n_cands][2] (hor, ver, 1/16 pel) the PUs' cand_first / cand_count index into.  Returns a BI_BEST_DT array (each stage's
+        result: integer vector and uiBestSad, rcMvHalf / rcMvQter and the fractional ruiCost, the final rcMv, ruiBits and ruiCost)."""
+        pus = np.ascontiguousarray(pus, dtype=L.BI_PU_DT)
+        pred = np.ascontiguousarray(pred, dtype=np.int16)
+        assert pred.shape == (len(pus), h, w)
+        cands = np.zeros((0, 2), dtype=np.int32) if cands is None else np.ascontiguousarray(cands, dtype=np.int32).reshape(-1, 2)
+        out = np.zeros(len(pus), dtype=L.BI_BEST_DT)
+        self._chk(self.lib.vvb_bipred_search(self.h, org_plane, ref_plane, _p(pus), len(pus), w, h, ctypes.byref(par),
+                                             _p(cands) if len(cands) else None, len(cands), _p(pred), _p(out)))
         return out
 
     # ---- dependent quantisation

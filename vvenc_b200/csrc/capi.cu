@@ -23,6 +23,7 @@
 #include "mctf_control_kernels.cuh"
 #include "tz_kernels.cuh"
 #include "frac_search_kernels.cuh"
+#include "bipred_kernels.cuh"
 #include "depquant_host.h"
 #include "rdoq_host.h"
 #include "vvc_tables.h"
@@ -424,7 +425,8 @@ int vvb_create( vvb_ctx** out, int device )
     VVB_RING_SMEM( 16 ), VVB_RING_SMEM( 32 ), VVB_RING_SMEM( 64 ),
     smemLimit( mctf_error_packed_kernel, 100 * 1024 ), smemLimit( mctf_grid_kernel, 200 * 1024 ), smemLimit( mctf_wave_kernel, 100 * 1024 ),
     smemLimit( mctf_int_grid_kernel, 100 * 1024 ), smemLimit( mctf_apply_kernel, 100 * 1024 ), smemLimit( frac_grid_kernel, 100 * 1024 ),
-    smemLimit( frac_grid_generic_kernel, 100 * 1024 ), smemLimit( frac_search_kernel, FRAC_SEARCH_SMEM ),
+    smemLimit( frac_grid_generic_kernel, 100 * 1024 ), smemLimit( frac_search_kernel<FracOrgPlane>, FRAC_SEARCH_SMEM ),
+    smemLimit( frac_search_kernel<FracOrgTarget, FracOrgTarget>, FRAC_SEARCH_SMEM ),
     VVB_FWD_TC_SMEM( 8 ), VVB_FWD_TC_SMEM( 16 ), VVB_FWD_TC_SMEM( 32 ), VVB_FWD_TC_SMEM( 64 ), VVB_ITC_SMEM( 8 ), VVB_ITC_SMEM( 16 ), VVB_ITC_SMEM( 32 ), VVB_ITC_SMEM( 64 ) };
 #undef VVB_FWD_TC_SMEM
 #undef VVB_ITC_SMEM
@@ -2283,9 +2285,9 @@ int vvb_frac_search_dev( vvb_ctx* ctx, int orgPlane, int refPlane, const vvb_tz_
   const size_t smem = (size_t)( L.base + fp.slots * L.slotWords ) * 4;
   const int threads = w * h >= 64 * 64 ? 256 : 128;
   int perSm = 0;
-  CU( cudaOccupancyMaxActiveBlocksPerMultiprocessor( &perSm, frac_search_kernel, threads, smem ) );
+  CU( cudaOccupancyMaxActiveBlocksPerMultiprocessor( &perSm, frac_search_kernel<FracOrgPlane>, threads, smem ) );
   const int grid = (int) std::min<long long>( n, (long long) ctx->numSMs * std::max( 1, perSm ) );
-  frac_search_kernel<<<grid, threads, smem, ctx->stream>>>( ctx->planes.p[orgPlane], ctx->planes.p[refPlane], dPus, dIntMv, n, fp, flt, mpHalf, mpQter, dOut );
+  frac_search_kernel<FracOrgPlane><<<grid, threads, smem, ctx->stream>>>( ctx->planes.p[orgPlane], ctx->planes.p[refPlane], dPus, dIntMv, n, fp, flt, mpHalf, mpQter, dOut );
   CHECK_LAUNCH( "frac_search_kernel" );
   return VVB_OK;
 }
@@ -2306,6 +2308,106 @@ int vvb_frac_search( vvb_ctx* ctx, int orgPlane, int refPlane, const vvb_tz_pu* 
   const vvb_tz_pu* dP; const vvb_tz_best* dM; vvb_frac_best* dO;
   return HostCall( ctx ).in( dP, pus, n ).in( dM, intMv, n ).out( dO, out, n )
                         .run( [&] { return vvb_frac_search_dev( ctx, orgPlane, refPlane, dP, dM, n, w, h, par, dO ); } );
+}
+
+// ---- bi-predictive refinement (the bBi branch of xMotionEstimation) ---------------------------------------------------------------------------
+static int bipredSetup( vvb_ctx* ctx, int orgPlane, int refPlane, int n, int w, int h, const vvb_bi_par* par, int nCands, TzPar& tp, MePar& mp, BiPar& bp,
+                        FracSearchPar& fp, FracFilter& flt, MePar& mpHalf, MePar& mpQter )
+{
+  if( !par || n < 0 || nCands < 0 ) return fail( ctx, VVB_ERR_ARG, "bad arguments" );
+  if( !validPlane( ctx, orgPlane ) || !validPlane( ctx, refPlane ) ) return fail( ctx, VVB_ERR_ARG, "unknown plane" );
+  if( par->search_range < 0 || par->search_range > VVB_BIPRED_MAX_RANGE || par->sub_shift_mode < 0 || par->sub_shift_mode > 2 || par->pic_w < 1 || par->pic_h < 1 ||
+      par->pic_w > 16384 || par->pic_h > 16384 || !isPow2( par->ctu_size ) || par->ctu_size < 16 || par->ctu_size > 128 || par->ifp_lines < 0 || par->ifp_lines > 1024 ||
+      ( par->ref_list != 0 && par->ref_list != 1 ) || par->fast_sub_pel < 0 || par->fast_sub_pel > 2 || par->reduce_tap < 0 || par->reduce_tap > 2 || par->imv < 0 || par->imv > 3 )
+    return fail( ctx, VVB_ERR_ARG, "bi-prediction settings out of range (search_range 0..VVB_BIPRED_MAX_RANGE, sub_shift_mode 0..2, ctu_size 16..128, ref_list 0..1, "
+                                   "fast_sub_pel 0..2, reduce_tap 0..2, imv 0..3)" );
+  if( !std::isfinite( par->lambda ) || par->lambda < 0 ) return fail( ctx, VVB_ERR_ARG, "lambda must be finite and not negative" );
+  if( par->imv == 1 || par->imv == 2 ) return fail( ctx, VVB_ERR_UNSUPPORTED, "IMV_FPEL / IMV_4PEL refine with xPatternSearchIntRefine, which the call does not run" );
+  if( par->dfunc != VVB_DF_SAD && par->dfunc != VVB_DF_HAD && par->dfunc != VVB_DF_HAD_FAST ) return fail( ctx, VVB_ERR_UNSUPPORTED, "bi-prediction search: SAD, HAD or HAD_fast" );
+  if( !isPow2( w ) || !isPow2( h ) || w < 4 || h < 4 || w > 128 || h > 128 || w * h < 64 )
+    return fail( ctx, VVB_ERR_UNSUPPORTED, "bi-prediction search: PU sides 4..128, powers of two, not 4x4, 4x8 or 8x4 (CU::isBipredRestriction)" );
+  if( w > par->ctu_size || h > par->ctu_size ) return fail( ctx, VVB_ERR_UNSUPPORTED, "bi-prediction search PUs no larger than the CTU" );
+  // the member's AVX2 SAD of widths >= 64 returns a partial sum once it passes maximumDistortionForEarlyExit (RdCostX86.h:372-405), and xPatternRefinement
+  // keeps those partial sums in distH, from which m_fastSubPel = 1 derives its pattern id (InterSearch.cpp:872-880, 886-969): not decision-equivalent there
+  if( par->dfunc == VVB_DF_SAD && par->fast_sub_pel == 1 && w >= 64 )
+    return fail( ctx, VVB_ERR_UNSUPPORTED, "bi-prediction search: SAD with fast_sub_pel 1 needs w < 64 (the member's early-exit partial sums enter the pattern id)" );
+  const Plane &op = ctx->planes.p[orgPlane], &rp = ctx->planes.p[refPlane];
+  if( op.bitDepth > 12 || rp.bitDepth > 12 ) return fail( ctx, VVB_ERR_UNSUPPORTED, "bi-prediction search: planes of up to 12 bits" );
+  if( w > par->pic_w || h > par->pic_h || op.width < par->pic_w || op.height < par->pic_h ) return fail( ctx, VVB_ERR_UNSUPPORTED, "the original plane or the picture is smaller than the PUs" );
+  const vvb_me_par me{ par->lambda, 2, par->imv == 3 ? 1 : 0, 0, 0, 0, 0 };          // cost scale 2 (:2043), imvShift (:2020)
+  int rc = makeMePar( ctx, &me, mp );
+  if( rc ) return rc;
+  int subShift = 0;
+  if( par->sub_shift_mode == 1 && h > 8 && w <= 128 ) subShift = 1;        // RdCost::setDistParam (RdCost.cpp:185-200)
+  if( par->sub_shift_mode == 2 && h > 8 ) subShift = 1;
+  mp.subShift = subShift;
+  tp = TzPar{};
+  tp.searchRange = par->search_range; tp.subShift = subShift;
+  tp.picW = par->pic_w; tp.picH = par->pic_h; tp.ctuSize = par->ctu_size; tp.ctuLog2 = ilog2h( par->ctu_size );
+  tp.heightInCtus = ( par->pic_h + par->ctu_size - 1 ) / par->ctu_size; tp.ifpLines = par->ifp_lines;
+  tp.w = w; tp.h = h; tp.nCands = nCands;
+  bp.clip = par->clip != 0; bp.maxv = ( 1 << op.bitDepth ) - 1; bp.imvShift = me.imv_shift; bp.refList = par->ref_list;
+  bp.motionLambda = std::sqrt( par->lambda );                                 // RdCost.cpp:77
+  if( par->fast_sub_pel == 2 ) return VVB_OK;
+  const vvb_frac_par fpar{ par->lambda, par->dfunc, par->reduce_tap, par->imv == 3, par->fast_sub_pel };
+  return fracSearchSetup( ctx, orgPlane, refPlane, n, w, h, &fpar, fp, flt, mpHalf, mpQter );
+}
+
+int vvb_bipred_search_dev( vvb_ctx* ctx, int orgPlane, int refPlane, const vvb_bi_pu* dPus, int n, int w, int h, const vvb_bi_par* par,
+                           const int32_t* dCands, int nCands, const int16_t* dPred, vvb_bi_best* dOut )
+{
+  if( !ctx || !dPus || !dPred || !dOut || ( nCands > 0 && !dCands ) ) return fail( ctx, VVB_ERR_ARG, "bad arguments" );
+  TzPar tp; MePar mp, mpHalf, mpQter; BiPar bp; FracSearchPar fp; FracFilter flt;
+  int rc = bipredSetup( ctx, orgPlane, refPlane, n, w, h, par, nCands, tp, mp, bp, fp, flt, mpHalf, mpQter );
+  if( rc || n == 0 ) return rc;
+  CU( cudaSetDevice( ctx->device ) );
+  vvb_tz_best* dInt;
+  if( ( rc = scratch( ctx, ScratchArena::Work, (size_t) n * sizeof( vvb_tz_best ), (void**) &dInt ) ) ) return rc;
+  const Plane &op = ctx->planes.p[orgPlane], &rp = ctx->planes.p[refPlane];
+  const int finish = par->fast_sub_pel == 2;
+  {
+    const int G = pick_group( FAM_SAD, w, h >> tp.subShift );
+    void ( *kernel )( const Plane, const Plane, const vvb_bi_pu*, int, const int32_t*, const int16_t*, const TzPar, const MePar, const BiPar, int, vvb_tz_best*, vvb_bi_best* ) =
+      G == 4 ? bipred_int_kernel<4> : G == 8 ? bipred_int_kernel<8> : G == 16 ? bipred_int_kernel<16> : bipred_int_kernel<32>;
+    const int perWarp = tz_warp_smem( w, h ), wpc = std::max( 1, std::min( 4, ( 48 * 1024 ) / perWarp ) );
+    const size_t smem = (size_t) wpc * perWarp;
+    int perSm = 0;
+    CU( cudaOccupancyMaxActiveBlocksPerMultiprocessor( &perSm, kernel, wpc * 32, smem ) );
+    const int grid = (int) std::min<long long>( ( n + wpc - 1 ) / wpc, (long long) ctx->numSMs * std::max( 1, perSm ) );
+    kernel<<<grid, wpc * 32, smem, ctx->stream>>>( op, rp, dPus, n, dCands, dPred, tp, mp, bp, finish, dInt, dOut );
+    CHECK_LAUNCH( "bipred_int_kernel" );
+  }
+  if( finish ) return VVB_OK;
+  const FracSearchSmem L = frac_search_smem( w, h );
+  const size_t smem = (size_t)( L.base + fp.slots * L.slotWords ) * 4;
+  const int threads = w * h >= 64 * 64 ? 256 : 128;
+  int perSm = 0;
+  CU( cudaOccupancyMaxActiveBlocksPerMultiprocessor( &perSm, frac_search_kernel<FracOrgTarget, FracOrgTarget>, threads, smem ) );
+  const int grid = (int) std::min<long long>( n, (long long) ctx->numSMs * std::max( 1, perSm ) );
+  frac_search_kernel<FracOrgTarget, FracOrgTarget><<<grid, threads, smem, ctx->stream>>>( op, rp, dPus, dInt, n, fp, flt, mpHalf, mpQter, dOut, FracOrgTarget{ dPred, w * h, bp } );
+  CHECK_LAUNCH( "frac_search_kernel<FracOrgTarget>" );
+  return VVB_OK;
+}
+
+int vvb_bipred_search( vvb_ctx* ctx, int orgPlane, int refPlane, const vvb_bi_pu* pus, int n, int w, int h, const vvb_bi_par* par,
+                       const int32_t* cands, int nCands, const int16_t* pred, vvb_bi_best* out )
+{
+  if( !ctx || !pus || !pred || !out || ( nCands > 0 && !cands ) ) return fail( ctx, VVB_ERR_ARG, "bad arguments" );
+  TzPar tp; MePar mp, mpHalf, mpQter; BiPar bp; FracSearchPar fp; FracFilter flt;
+  int rc = bipredSetup( ctx, orgPlane, refPlane, n, w, h, par, nCands, tp, mp, bp, fp, flt, mpHalf, mpQter );
+  if( rc || n == 0 ) return rc;
+  const Plane& rp = ctx->planes.p[refPlane];
+  for( int i = 0; i < n; i++ )
+  {
+    const vvb_bi_pu& p = pus[i];
+    if( p.x < 0 || p.y < 0 || p.x > par->pic_w - w || p.y > par->pic_h - h ) return fail( ctx, VVB_ERR_ARG, "PU outside the picture" );
+    if( p.cand_first < 0 || p.cand_count < 0 || p.cand_first > nCands - p.cand_count ) return fail( ctx, VVB_ERR_ARG, "candidate range outside cands" );
+    if( p.bcw_idx < 0 || p.bcw_idx > 4 ) return fail( ctx, VVB_ERR_ARG, "bcw_idx outside 0..4" );
+    if( !bi_admitted( tp, rp, p, cands ) ) return fail( ctx, VVB_ERR_UNSUPPORTED, "read box outside the reference margin (see vvb_bipred_search in the header)" );
+  }
+  const vvb_bi_pu* dP; const int32_t* dC; const int16_t* dPr; vvb_bi_best* dO;
+  return HostCall( ctx ).in( dP, pus, n ).in( dC, cands, (size_t) 2 * nCands ).in( dPr, pred, (size_t) n * w * h ).out( dO, out, n )
+                        .run( [&] { return vvb_bipred_search_dev( ctx, orgPlane, refPlane, dP, n, w, h, par, dC, nCands, dPr, dO ); } );
 }
 
 // ---- MCTF apply stage (xFinalizeBlkLine body per block) ---------------------------------------------------------------------

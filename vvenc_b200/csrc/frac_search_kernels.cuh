@@ -178,10 +178,26 @@ struct FracSearchCta
   }
 };
 
+// Where frac_search_kernel's PUs, original block and results come from.  FracOrgPlane: vvb_frac_search -- vvb_tz_search's PU list, the PU's block of the
+// original plane, vvb_frac_best.  (bipred_kernels.cuh has the other source: the bi-prediction target 2 * org - pred.)
+struct FracOrgPlane
+{
+  using Pu = vvb_tz_pu;
+  using Out = vvb_frac_best;
+  // the original pels ( 2 * i, 2 * i + 1 ) of PU b's compact block, q pointing at the first of them in the plane
+  __device__ __forceinline__ uint32_t org_pair( const int16_t* q, int, int ) const { return (uint32_t)(uint16_t) __ldg( q ) | ( (uint32_t)(uint16_t) __ldg( q + 1 ) << 16 ); }
+  __device__ __forceinline__ void fail( Out* out, int b ) const { vvb_frac_best r{}; r.cost = ~0ull; out[b] = r; }
+  __device__ __forceinline__ void done( Out* out, int b, const Pu&, int, int, const vvb_frac_best& r ) const { out[b] = r; }
+};
+
+// Src: where the PUs, the original block and the results come from.  Extra: the kernel parameters Src is built from -- none for FracOrgPlane, so its
+// instantiation keeps the parameter list and the code of the kernel before Src existed.
+template<class Src, class... Extra>
 __global__ void __launch_bounds__( 256, 2 ) frac_search_kernel( const __grid_constant__ Plane orgPlane, const __grid_constant__ Plane refPlane,
-                                                             const vvb_tz_pu* __restrict__ pus, const vvb_tz_best* __restrict__ intMv, int n,
+                                                             const typename Src::Pu* __restrict__ pus, const vvb_tz_best* __restrict__ intMv, int n,
                                                              const __grid_constant__ FracSearchPar p, const __grid_constant__ FracFilter flt,
-                                                             const __grid_constant__ MePar mpHalf, const __grid_constant__ MePar mpQter, vvb_frac_best* __restrict__ out )
+                                                             const __grid_constant__ MePar mpHalf, const __grid_constant__ MePar mpQter, typename Src::Out* __restrict__ out,
+                                                             Extra... extra )
 {
   extern __shared__ __align__( 16 ) uint32_t sFs[];
   __shared__ uint32_t sMv[VVB_MVCOST_ENTRIES];
@@ -210,11 +226,11 @@ __global__ void __launch_bounds__( 256, 2 ) frac_search_kernel( const __grid_con
 
   for( int b = blockIdx.x; b < n; b += gridDim.x )
   {
-    const vvb_tz_pu pu = pus[b];
+    const typename Src::Pu pu = pus[b];
     const int mx = intMv[b].mv_hor, my = intMv[b].mv_ver;
     if( pu.x < 0 || pu.y < 0 || pu.x > orgPlane.width - w || pu.y > orgPlane.height - h || !frac_search_admitted( refPlane, pu.x, pu.y, mx, my, w, h ) )
     {
-      if( tid == 0 ) { vvb_frac_best r{}; r.cost = ~0ull; out[b] = r; }
+      if( tid == 0 ) Src{ extra... }.fail( out, b );
       continue;
     }
     __syncthreads();                         // the previous PU is done with the shared buffers
@@ -227,7 +243,7 @@ __global__ void __launch_bounds__( 256, 2 ) frac_search_kernel( const __grid_con
       {
         const int y = div_rcp( i, invHw ), c = i - y * hw;
         const int16_t* q = src + (ptrdiff_t) y * orgPlane.stride + 2 * c;
-        orgW[i] = (uint32_t)(uint16_t) __ldg( q ) | ( (uint32_t)(uint16_t) __ldg( q + 1 ) << 16 );
+        orgW[i] = Src{ extra... }.org_pair( q, b, i );
       }
     }
     if( tid < 18 ) sDist[tid] = 0u;
@@ -292,7 +308,7 @@ __global__ void __launch_bounds__( 256, 2 ) frac_search_kernel( const __grid_con
       r.half_hor = c_refineH[dir][0]; r.half_ver = c_refineH[dir][1];
       r.qter_hor = c_refineQ[qdir][0]; r.qter_ver = c_refineQ[qdir][1];
       r.cost = best;
-      out[b] = r;
+      Src{ extra... }.done( out, b, pu, mx, my, r );
     }
   }
 }

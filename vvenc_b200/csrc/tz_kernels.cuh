@@ -35,7 +35,7 @@ static_assert( sizeof( vvb_tz_pu ) == 28 && sizeof( vvb_tz_best ) == 32, "vvb_tz
 struct TzClip { int horMin, horMax, verMin, verMax; };
 
 // clipMv (CommonLib/Mv.cpp:68-80) and xClipMvSearch (InterSearch.cpp:2134-2152): limits in 1/16 pel
-__device__ __forceinline__ TzClip tz_clip_box( const TzPar& p, int x, int y, bool search )
+__host__ __device__ __forceinline__ TzClip tz_clip_box( const TzPar& p, int x, int y, bool search )
 {
   TzClip c;
   c.horMax = ( p.picW + 8 - x - 1 ) << 4;
@@ -47,9 +47,22 @@ __device__ __forceinline__ TzClip tz_clip_box( const TzPar& p, int x, int y, boo
   c.verMin = ( -p.ctuSize - 8 - y + 1 ) * 16;
   return c;
 }
-__device__ __forceinline__ int tz_clamp( int v, int lo, int hi ) { return min( hi, max( lo, v ) ); }
+__host__ __device__ __forceinline__ int tz_clamp( int v, int lo, int hi ) { return min( hi, max( lo, v ) ); }
 // Mv::changePrecision to a coarser precision and Mv::divideByPowerOf2 (Mv.h:134-142, 189-203): the same rounding
-__device__ __forceinline__ int tz_round_shift( int v, int s ) { const int o = 1 << ( s - 1 ); return v >= 0 ? ( v + o - 1 ) >> s : ( v + o ) >> s; }
+__host__ __device__ __forceinline__ int tz_round_shift( int v, int s ) { const int o = 1 << ( s - 1 ); return v >= 0 ? ( v + o - 1 ) >> s : ( v + o ) >> s; }
+
+// xSetSearchRange (InterSearch.cpp:2183-2206): the integer window of range rng around mv (1/16 pel), its top left clipped by clipMv, its bottom right
+// by xClipMvSearch
+__host__ __device__ __forceinline__ void tz_search_range( const TzPar& p, int x, int y, int mvHor, int mvVer, int rng, int& left, int& right, int& top, int& bottom )
+{
+  const TzClip cm = tz_clip_box( p, x, y, false ), cs = tz_clip_box( p, x, y, true );
+  const int r = rng << 4;
+  const int px = tz_clamp( mvHor, cm.horMin, cm.horMax ), py = tz_clamp( mvVer, cm.verMin, cm.verMax );
+  left   = tz_round_shift( tz_clamp( px - r, cm.horMin, cm.horMax ), 4 );
+  top    = tz_round_shift( tz_clamp( py - r, cm.verMin, cm.verMax ), 4 );
+  right  = tz_round_shift( tz_clamp( px + r, cs.horMin, cs.horMax ), 4 );
+  bottom = tz_round_shift( tz_clamp( py + r, cs.verMin, cs.verMax ), 4 );
+}
 
 struct TzState
 {
@@ -253,15 +266,7 @@ __global__ void __launch_bounds__( 128 ) tz_search_kernel( const __grid_constant
     T.flush();
 
     // xSetSearchRange around the best vector (:2372-2377)
-    {
-      const TzClip cm = tz_clip_box( p, pu.x, pu.y, false );
-      const int rng = ( p.searchRange >> ( p.fast ? 1 : 0 ) ) << 4;
-      const int px = tz_clamp( s.bestX * 16, cm.horMin, cm.horMax ), py = tz_clamp( s.bestY * 16, cm.verMin, cm.verMax );
-      s.left   = tz_round_shift( tz_clamp( px - rng, cm.horMin, cm.horMax ), 4 );
-      s.top    = tz_round_shift( tz_clamp( py - rng, cm.verMin, cm.verMax ), 4 );
-      s.right  = tz_round_shift( tz_clamp( px + rng, cs.horMin, cs.horMax ), 4 );
-      s.bottom = tz_round_shift( tz_clamp( py + rng, cs.verMin, cs.verMax ), 4 );
-    }
+    tz_search_range( p, pu.x, pu.y, s.bestX * 16, s.bestY * 16, p.searchRange >> ( p.fast ? 1 : 0 ), s.left, s.right, s.top, s.bottom );
 
     const bool ext = p.extended != 0;
     bool done = false;
