@@ -153,7 +153,7 @@ __global__ void __launch_bounds__( 128 ) frac_grid_kernel( const __grid_constant
           d[8*r+6] = lo16( ow.w ) - d[8*r+6]; d[8*r+7] = hi16( ow.w ) - d[8*r+7];
         }
         uint32_t s = 0;
-        if( family == 2 ) s = had8( d );
+        if( family == 2 ) s = had8<0, 1>( d );          // one abs-sum chain: with four, ptxas spills in this kernel
         else
         {
 #pragma unroll
