@@ -12,38 +12,19 @@ import argparse
 import ctypes
 import json
 import os
-import subprocess
 import sys
 import time
 
 import numpy as np
 
+from me_bench_common import PW, PH, card, pictures, timed
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'tests'))
 
-PW, PH, CTU, LAM, RANGE = 3840, 2160, 128, 57.25, 384
+CTU, LAM, RANGE = 128, 57.25, 384
 MARGIN = CTU + 12                  # the margin the header states for every vector the clip rules allow
 SHAPES = (8, 16, 32, 64, 128)
-
-
-def card():
-    try:
-        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, plim = [s.strip() for s in q.split(',')]
-        return name, plim
-    except Exception as e:                    # noqa: BLE001
-        return 'unknown (%s)' % e, 'unknown'
-
-
-def pictures():
-    rs = np.random.RandomState(2160)
-    S = PW + 2 * MARGIN
-    b = rs.randint(0, 1024, size=(PH + 2 * MARGIN + 8, S + 8))
-    sm = (b + np.roll(b, 1, 0) + np.roll(b, 1, 1) + np.roll(b, (1, 1), (0, 1))) // 4
-    org = np.ascontiguousarray(sm[4:4 + PH + 2 * MARGIN, 4:4 + S], dtype=np.int16)
-    cur = np.ascontiguousarray(np.clip(sm[1:1 + PH + 2 * MARGIN, 7:7 + S] + rs.randint(-9, 10, size=org.shape), 0, 1023), dtype=np.int16)
-    oth = np.ascontiguousarray(np.clip(sm[6:6 + PH + 2 * MARGIN, 2:2 + S] + rs.randint(-9, 10, size=org.shape), 0, 1023), dtype=np.int16)
-    return org, cur, oth, S
 
 
 def main():
@@ -54,7 +35,7 @@ def main():
     import vvenc_b200 as V
     import test_gpu_bipred_search as T
     name, plim = card()
-    org, cur, oth, S = pictures()
+    org, cur, oth, S = pictures(MARGIN, third=True)
     eng = V.CostEngine(0)
     eng.upload_plane(0, org, PW, PH, MARGIN, bit_depth=10); eng.upload_plane(1, cur, PW, PH, MARGIN, bit_depth=10)
     from _libs import refshim
@@ -62,15 +43,6 @@ def main():
     stream = torch.cuda.ExternalStream(eng.stream)
     vp = ctypes.c_void_p
     T.LAM = LAM
-
-    def timed(fn, reps):
-        fn(); eng.synchronize()
-        t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        t0.record(stream)
-        for _ in range(reps):
-            fn()
-        t1.record(stream); t1.synchronize()
-        return t0.elapsed_time(t1) / reps
 
     # start vectors from the uni chain, left on the device
     rs = np.random.RandomState(4096)
@@ -120,8 +92,8 @@ def main():
                                                  vp(j['d_out'].data_ptr())) == 0
         row = {'search_range': rng, 'bipred_ms': {}, 'member_ms': {}, 'mismatches': {}}
         for s in SHAPES:
-            row['bipred_ms'][s] = round(timed(lambda: run(s), a.reps), 3)
-        row['bipred_picture_ms'] = round(timed(lambda: [run(s) for s in SHAPES], a.reps), 3)
+            row['bipred_ms'][s] = round(timed(eng, stream, lambda: run(s), a.reps), 3)
+        row['bipred_picture_ms'] = round(timed(eng, stream, lambda: [run(s) for s in SHAPES], a.reps), 3)
         for s in SHAPES:
             run(s)
         eng.synchronize()

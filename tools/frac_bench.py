@@ -11,37 +11,19 @@ import argparse
 import ctypes
 import json
 import os
-import subprocess
 import sys
 import time
 
 import numpy as np
 
+from me_bench_common import PW, PH, card, pictures, timed
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'tests'))
 
-PW, PH, CTU, LAM, RANGE = 3840, 2160, 128, 57.0, 384
+CTU, LAM, RANGE = 128, 57.0, 384
 MARGIN = CTU + 12                  # the margin the header states for every vector vvb_tz_search can return
 SHAPES = (8, 16, 32, 64, 128)
-
-
-def card():
-    try:
-        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, plim = [s.strip() for s in q.split(',')]
-        return name, plim
-    except Exception as e:                    # noqa: BLE001
-        return 'unknown (%s)' % e, 'unknown'
-
-
-def pictures():
-    rs = np.random.RandomState(2160)
-    S = PW + 2 * MARGIN
-    b = rs.randint(0, 1024, size=(PH + 2 * MARGIN + 8, S + 8))
-    sm = (b + np.roll(b, 1, 0) + np.roll(b, 1, 1) + np.roll(b, (1, 1), (0, 1))) // 4
-    org = np.ascontiguousarray(sm[4:4 + PH + 2 * MARGIN, 4:4 + S], dtype=np.int16)
-    cur = np.ascontiguousarray(np.clip(sm[1:1 + PH + 2 * MARGIN, 7:7 + S] + rs.randint(-9, 10, size=org.shape), 0, 1023), dtype=np.int16)
-    return org, cur, S
 
 
 def main():
@@ -52,7 +34,7 @@ def main():
     import vvenc_b200 as V
     from _libs import refshim, P, PO
     name, plim = card()
-    org, cur, S = pictures()
+    org, cur, S = pictures(MARGIN)
     base = MARGIN * S + MARGIN
     eng = V.CostEngine(0)
     eng.upload_plane(0, org, PW, PH, MARGIN, bit_depth=10); eng.upload_plane(1, cur, PW, PH, MARGIN, bit_depth=10)
@@ -62,15 +44,6 @@ def main():
     R.refshim_set_simd(b'AVX2')
     stream = torch.cuda.ExternalStream(eng.stream)
     vp = ctypes.c_void_p
-
-    def timed(fn, reps):
-        fn(); eng.synchronize()
-        t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        t0.record(stream)
-        for _ in range(reps):
-            fn()
-        t1.record(stream); t1.synchronize()
-        return t0.elapsed_time(t1) / reps
 
     # integer vectors: vvb_tz_search_dev with the medium settings, left on the device
     rs = np.random.RandomState(4096)
@@ -121,14 +94,14 @@ def main():
 
         row = {'fast_sub_pel': fast, 'frac_ms': {}, 'grid_ms': {}, 'd2h_ms': {}, 'member_ms': {}, 'mismatches': {}}
         for s in SHAPES:
-            row['frac_ms'][s] = round(timed(lambda: frac(s), a.reps), 3)
+            row['frac_ms'][s] = round(timed(eng, stream, lambda: frac(s), a.reps), 3)
             if s <= 64:
-                row['grid_ms'][s] = round(timed(lambda: grid(s), a.reps), 3)
+                row['grid_ms'][s] = round(timed(eng, stream, lambda: grid(s), a.reps), 3)
                 with torch.cuda.stream(stream):
-                    row['d2h_ms'][s] = round(timed(lambda: d2h(s), a.reps), 3)
-        row['frac_picture_ms'] = round(timed(lambda: [frac(s) for s in SHAPES], a.reps), 3)
-        row['grid_picture_ms_le64'] = round(timed(lambda: [grid(s) for s in SHAPES if s <= 64], a.reps), 3)
-        row['frac_picture_ms_le64'] = round(timed(lambda: [frac(s) for s in SHAPES if s <= 64], a.reps), 3)
+                    row['d2h_ms'][s] = round(timed(eng, stream, lambda: d2h(s), a.reps), 3)
+        row['frac_picture_ms'] = round(timed(eng, stream, lambda: [frac(s) for s in SHAPES], a.reps), 3)
+        row['grid_picture_ms_le64'] = round(timed(eng, stream, lambda: [grid(s) for s in SHAPES if s <= 64], a.reps), 3)
+        row['frac_picture_ms_le64'] = round(timed(eng, stream, lambda: [frac(s) for s in SHAPES if s <= 64], a.reps), 3)
         for s in SHAPES:
             frac(s)
         eng.synchronize()

@@ -18,33 +18,16 @@ from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
+from me_bench_common import PW, PH, card, pictures, timed
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'tests'))
 
-PW, PH, MARGIN, CTU, LAM = 3840, 2160, 144, 128, 57.0
+MARGIN, CTU, LAM = 144, 128, 57.0
 # The dense-table binding cannot run SearchRange 384 here: the window of a 64x64 PU (the range clamped to the binding's reach, 145 x 145 positions) needs
 # 233 920 bytes of shared memory in vvb_sad_search, above its 220 KB limit, so the call answers VVB_ERR_UNSUPPORTED; B200RowSearch::runTables turns that into a
 # THROW, and composing that exception's message faults inside the reference probe library (vvenc::Exception::operator<< -> std::ostream::_M_insert<long>).
 TABLE_NOT_MEASURED = {384: 'the 64x64 table window exceeds vvb_sad_search shared memory; the binding error path faults in the probe library (DESIGN §5)'}
-
-
-def card():
-    try:
-        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, plim = [s.strip() for s in q.split(',')]
-        return name, plim
-    except Exception as e:                    # noqa: BLE001
-        return 'unknown (%s)' % e, 'unknown'
-
-
-def pictures():
-    rs = np.random.RandomState(2160)
-    S = PW + 2 * MARGIN
-    b = rs.randint(0, 1024, size=(PH + 2 * MARGIN + 8, S + 8))
-    sm = (b + np.roll(b, 1, 0) + np.roll(b, 1, 1) + np.roll(b, (1, 1), (0, 1))) // 4
-    org = np.ascontiguousarray(sm[4:4 + PH + 2 * MARGIN, 4:4 + S], dtype=np.int16)
-    cur = np.ascontiguousarray(np.clip(sm[1:1 + PH + 2 * MARGIN, 7:7 + S] + rs.randint(-9, 10, size=org.shape), 0, 1023), dtype=np.int16)
-    return org, cur, S
 
 
 def pu_lists():
@@ -67,7 +50,7 @@ def table_leg(rng, sample):
     """refshim_tz_search_rows_b200 bound to the real library on `sample` PUs per shape, scaled to the picture; prints {"table_ms_scaled": ...}"""
     import vvenc_b200 as V
     from _libs import refshim, P, PO
-    org, cur, S = pictures()
+    org, cur, S = pictures(MARGIN)
     R = refshim()
     R.refshim_tz_search_rows_b200.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                               ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double] + [ctypes.c_int] * 7 + [ctypes.c_void_p]
@@ -99,7 +82,7 @@ def main():
     import vvenc_b200 as V
     from _libs import refshim, P, PO
     name, plim = card()
-    org, cur, S = pictures()
+    org, cur, S = pictures(MARGIN)
     lists = pu_lists()
     eng = V.CostEngine(0)
     eng.upload_plane(0, org, PW, PH, MARGIN, bit_depth=10); eng.upload_plane(1, cur, PW, PH, MARGIN, bit_depth=10)
@@ -130,13 +113,7 @@ def main():
             for s, blk in lists.items():
                 rc = eng.lib.vvb_tz_search_dev(eng.h, 0, 1, d_pus[s].data_ptr(), len(blk), s, s, ctypes.byref(me), ctypes.byref(tz), None, 0, d_out[s].data_ptr())
                 assert rc == 0, eng.lib.vvb_last_error(eng.h)
-        picture(); eng.synchronize()
-        t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        t0.record(stream)
-        for _ in range(a.reps):
-            picture()
-        t1.record(stream); t1.synchronize()
-        dev_ms = t0.elapsed_time(t1) / a.reps
+        dev_ms = timed(eng, stream, picture, a.reps)
         print('device: range %d %.3f ms' % (rng, dev_ms), file=sys.stderr, flush=True)
         # the member on all host threads; its results check the device's
         member_ms = 0.0; mismatched = 0

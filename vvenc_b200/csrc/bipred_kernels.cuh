@@ -106,23 +106,14 @@ __global__ void __launch_bounds__( 128, 1 ) bipred_int_kernel( const __grid_cons
 {
   extern __shared__ __align__( 16 ) uint8_t biSmem[];
   __shared__ uint32_t sMv[VVB_MVCOST_ENTRIES];
-  for( int i = threadIdx.x; i < VVB_MVCOST_ENTRIES; i += blockDim.x ) sMv[i] = mp.tab.cost[i];
-  __syncthreads();
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  uint8_t* mine = biSmem + (size_t) warp * tz_warp_smem( p.w, p.h );
-  int16_t* tgt = reinterpret_cast<int16_t*>( mine );
-  TzWarp W;
-  W.org = tgt;
-  W.pts = reinterpret_cast<int4*>( mine + ( ( p.w * p.h * 2 + 15 ) & ~15 ) );
-  W.sad = reinterpret_cast<uint32_t*>( W.pts + TZ_LIST );
-  W.refStride = refPlane.stride; W.lane = lane; W.cnt = 0;
-  const int warpsPerGrid = gridDim.x * ( blockDim.x >> 5 );
+  TzWarp W = tz_warp_begin( biSmem, sMv, p, mp, refPlane );
+  int16_t* tgt = W.org;
+  const int lane = W.lane, warp = threadIdx.x >> 5, warpsPerGrid = gridDim.x * ( blockDim.x >> 5 );
 
-  for( int i = blockIdx.x * ( blockDim.x >> 5 ) + warp; i < n; i += warpsPerGrid )
+  for( int i = blockIdx.x * ( blockDim.x >> 5 ) + warp; i < n; i += warpsPerGrid )     // persistent warps, as tz_search_kernel
   {
     const vvb_bi_pu pu = pus[i];
-    if( pu.x < 0 || pu.y < 0 || pu.x > p.picW - p.w || pu.y > p.picH - p.h || pu.cand_first < 0 || pu.cand_count < 0 || pu.cand_first > p.nCands - pu.cand_count ||
-        pu.bcw_idx < 0 || pu.bcw_idx > 4 || !bi_admitted( p, refPlane, pu, cands ) )
+    if( TZ_PU_OUTSIDE( p, pu ) || pu.bcw_idx < 0 || pu.bcw_idx > 4 || !bi_admitted( p, refPlane, pu, cands ) )
     {
       if( lane == 0 ) { vvb_tz_best t{}; t.mv_hor = t.mv_ver = BI_REFUSED_MV; intOut[i] = t; out[i] = bi_sentinel(); }
       continue;
@@ -137,8 +128,7 @@ __global__ void __launch_bounds__( 128, 1 ) bipred_int_kernel( const __grid_cons
     W.ref = refPlane.origin + (ptrdiff_t) pu.y * refPlane.stride + pu.x;
 
     TzState s;
-    s.bestSad = ~0ull; s.bestX = 0; s.bestY = 0; s.bestDistance = 0; s.bestRound = 0; s.pointNr = 0;
-    s.left = s.right = s.top = s.bottom = 0;
+    tz_reset( s );
     TzWalk<G> T{ W, s, p, mp, sMv, pu.pred_hor, pu.pred_ver };
     const TzClip cs = tz_clip_box( p, pu.x, pu.y, true );
 
@@ -160,15 +150,11 @@ __global__ void __launch_bounds__( 128, 1 ) bipred_int_kernel( const __grid_cons
     // xSetSearchRange around the unclipped winner, then xPatternSearch from uiSadBest = MAX_DISTORTION and (0, 0)
     int l, r, t, b;
     tz_search_range( p, pu.x, pu.y, initH, initV, p.searchRange, l, r, t, b );
-    s.bestSad = ~0ull; s.bestX = 0; s.bestY = 0;
+    tz_reset( s );
     T.raster( t, b, l, r, 1 );
     if( lane == 0 )
     {
-      vvb_tz_best ib;
-      ib.mv_hor = s.bestX; ib.mv_ver = s.bestY;
-      ib.cost = s.bestSad;
-      ib.sad = s.bestSad - mv_cost( mp, sMv, s.bestX, s.bestY, pu.pred_hor, pu.pred_ver );
-      ib.best_distance = 0; ib.pad = 0;
+      const vvb_tz_best ib = tz_best( s, mp, sMv, pu.pred_hor, pu.pred_ver, 0 );
       intOut[i] = ib;
       vvb_bi_best o = bi_sentinel();
       o.int_hor = s.bestX; o.int_ver = s.bestY; o.int_best = s.bestSad;

@@ -73,10 +73,17 @@ struct TzState
   int left, right, top, bottom;     // TZSearchStruct::searchRange
 };
 
+// the start of a walk: no best cost yet, the zero vector, a zero search range
+__device__ __forceinline__ void tz_reset( TzState& s )
+{
+  s.bestSad = ~0ull; s.bestX = 0; s.bestY = 0; s.bestDistance = 0; s.bestRound = 0; s.pointNr = 0;
+  s.left = s.right = s.top = s.bottom = 0;
+}
+
 // one warp's view of the walk: the staged original, the point list, the SADs of the listed points
 struct TzWarp
 {
-  const int16_t* org;               // shared, w x h compact
+  int16_t* org;                     // shared, w x h compact
   int4* pts;                        // shared [TZ_LIST]: x, y, ucPointNr (-1: an extra start candidate), distance
   uint32_t* sad;                    // shared [TZ_LIST]
   const int16_t* ref;               // reference plane at the PU position
@@ -201,8 +208,43 @@ template<int G> struct TzWalk
 
 };
 
-// per warp: org block (w * h pels, rounded to 16 bytes), the point list and its SADs
-__host__ __device__ inline int tz_warp_smem( int w, int h ) { return ( ( w * h * 2 + 15 ) & ~15 ) + TZ_LIST * 16 + TZ_LIST * 4; }
+// per warp: org block (w * h pels, rounded to 16 bytes), the point list and its SADs; pts is the point list's offset, bytes the warp's share.  The rounding is
+// written out twice: with bytes = pts + ..., ptxas gives tz_search_kernel<8> 78 registers instead of 72.
+struct TzWarpSmem { int pts, bytes; };
+__host__ __device__ inline TzWarpSmem tz_warp_smem( int w, int h ) { return { ( w * h * 2 + 15 ) & ~15, ( ( w * h * 2 + 15 ) & ~15 ) + TZ_LIST * 16 + TZ_LIST * 4 }; }
+
+// The PUs a walk refuses: outside the picture, or a candidate range outside cands.  vvb_tz_pu and vvb_bi_pu name these fields alike; both kernels give such a
+// PU a sentinel and both host calls refuse it.  A macro rather than a bool function, because through a function ptxas gives tz_search_kernel<4> and <8> 78
+// registers instead of 72.
+#define TZ_PU_OUTSIDE( p, pu ) ( (pu).x < 0 || (pu).y < 0 || (pu).x > (p).picW - (p).w || (pu).y > (p).picH - (p).h || (pu).cand_first < 0 || (pu).cand_count < 0 || \
+                                 (pu).cand_first > (p).nCands - (pu).cand_count )
+
+// the prologue of a warp-per-PU kernel: the CTA copies the MV-rate table to sMv, and each warp takes its share of the dynamic shared memory
+__device__ __forceinline__ TzWarp tz_warp_begin( uint8_t* smem, uint32_t* sMv, const TzPar& p, const MePar& mp, const Plane& refPlane )
+{
+  for( int i = threadIdx.x; i < VVB_MVCOST_ENTRIES; i += blockDim.x ) sMv[i] = mp.tab.cost[i];
+  __syncthreads();
+  const TzWarpSmem L = tz_warp_smem( p.w, p.h );
+  const int warp = threadIdx.x >> 5;
+  uint8_t* mine = smem + (size_t) warp * L.bytes;
+  TzWarp W;
+  W.org = reinterpret_cast<int16_t*>( mine );
+  W.pts = reinterpret_cast<int4*>( mine + L.pts );
+  W.sad = reinterpret_cast<uint32_t*>( W.pts + TZ_LIST );
+  W.refStride = refPlane.stride; W.lane = threadIdx.x & 31; W.cnt = 0;
+  return W;
+}
+
+// the result of a finished walk: its best vector and cost, and the SAD without the vector's MV rate
+__device__ __forceinline__ vvb_tz_best tz_best( const TzState& s, const MePar& mp, const uint32_t* tab, int predHor, int predVer, uint32_t bestDistance )
+{
+  vvb_tz_best b;
+  b.mv_hor = s.bestX; b.mv_ver = s.bestY;
+  b.cost = s.bestSad;
+  b.sad = s.bestSad - mv_cost( mp, tab, s.bestX, s.bestY, predHor, predVer );
+  b.best_distance = bestDistance; b.pad = 0;
+  return b;
+}
 
 template<int G>
 __global__ void __launch_bounds__( 128 ) tz_search_kernel( const __grid_constant__ Plane orgPlane, const __grid_constant__ Plane refPlane,
@@ -211,22 +253,14 @@ __global__ void __launch_bounds__( 128 ) tz_search_kernel( const __grid_constant
 {
   extern __shared__ __align__( 16 ) uint8_t tzSmem[];
   __shared__ uint32_t sMv[VVB_MVCOST_ENTRIES];
-  for( int i = threadIdx.x; i < VVB_MVCOST_ENTRIES; i += blockDim.x ) sMv[i] = mp.tab.cost[i];
-  __syncthreads();
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  uint8_t* mine = tzSmem + (size_t) warp * tz_warp_smem( p.w, p.h );
-  int16_t* org = reinterpret_cast<int16_t*>( mine );
-  TzWarp W;
-  W.org = org;
-  W.pts = reinterpret_cast<int4*>( mine + ( ( p.w * p.h * 2 + 15 ) & ~15 ) );
-  W.sad = reinterpret_cast<uint32_t*>( W.pts + TZ_LIST );
-  W.refStride = refPlane.stride; W.lane = lane; W.cnt = 0;
-  const int warpsPerGrid = gridDim.x * ( blockDim.x >> 5 );
+  TzWarp W = tz_warp_begin( tzSmem, sMv, p, mp, refPlane );
+  int16_t* org = W.org;
+  const int lane = W.lane, warp = threadIdx.x >> 5, warpsPerGrid = gridDim.x * ( blockDim.x >> 5 );
 
-  for( int i = blockIdx.x * ( blockDim.x >> 5 ) + warp; i < n; i += warpsPerGrid )
+  for( int i = blockIdx.x * ( blockDim.x >> 5 ) + warp; i < n; i += warpsPerGrid )     // persistent warps: PUs i, i + warps of the grid, ...
   {
     const vvb_tz_pu pu = pus[i];
-    if( pu.x < 0 || pu.y < 0 || pu.x > p.picW - p.w || pu.y > p.picH - p.h || pu.cand_first < 0 || pu.cand_count < 0 || pu.cand_first > p.nCands - pu.cand_count )
+    if( TZ_PU_OUTSIDE( p, pu ) )
     {
       if( lane == 0 ) { vvb_tz_best b{}; b.sad = ~0ull; b.cost = ~0ull; b.best_distance = 0xffffffffu; out[i] = b; }
       continue;
@@ -245,8 +279,7 @@ __global__ void __launch_bounds__( 128 ) tz_search_kernel( const __grid_constant
     W.ref = refPlane.origin + (ptrdiff_t) pu.y * refPlane.stride + pu.x;
 
     TzState s;
-    s.bestSad = ~0ull; s.bestX = 0; s.bestY = 0; s.bestDistance = 0; s.bestRound = 0; s.pointNr = 0;
-    s.left = s.right = s.top = s.bottom = 0;
+    tz_reset( s );
     TzWalk<G> T{ W, s, p, mp, sMv, pu.pred_hor, pu.pred_ver };
     const TzClip cs = tz_clip_box( p, pu.x, pu.y, true );
 
@@ -317,15 +350,7 @@ __global__ void __launch_bounds__( 128 ) tz_search_kernel( const __grid_constant
         if( s.bestDistance == 1 ) { s.bestDistance = 0; if( s.pointNr != 0 ) T.twoPoint(); }
       }
     }
-    if( lane == 0 )
-    {
-      vvb_tz_best b;
-      b.mv_hor = s.bestX; b.mv_ver = s.bestY;
-      b.cost = s.bestSad;
-      b.sad = s.bestSad - mv_cost( mp, sMv, s.bestX, s.bestY, pu.pred_hor, pu.pred_ver );
-      b.best_distance = s.bestDistance; b.pad = 0;
-      out[i] = b;
-    }
+    if( lane == 0 ) out[i] = tz_best( s, mp, sMv, pu.pred_hor, pu.pred_ver, s.bestDistance );
   }
 }
 
