@@ -42,6 +42,14 @@ class vvb_bi_par(ctypes.Structure):
                                                                           'clip', 'imv', 'fast_sub_pel', 'dfunc', 'reduce_tap')]
 
 
+class vvb_amvr_par(ctypes.Structure):
+    _fields_ = [('lam', ctypes.c_double), ('dfunc', ctypes.c_int32), ('imv', ctypes.c_int32), ('mvp_bits', ctypes.c_uint32 * 2)] + \
+               [(k, ctypes.c_int32) for k in ('pic_w', 'pic_h', 'ctu_size', 'ifp_lines')]
+
+
+AMVR_PAR = vvb_amvr_par
+
+
 class vvb_tu_par(ctypes.Structure):
     _fields_ = [('w', ctypes.c_int32), ('h', ctypes.c_int32), ('tr_hor', ctypes.c_int32), ('tr_ver', ctypes.c_int32), ('bit_depth', ctypes.c_int32),
                 ('qp', ctypes.c_int32), ('is_irap', ctypes.c_int32), ('dep_quant', ctypes.c_int32), ('sign_hiding', ctypes.c_int32), ('lfnst_idx', ctypes.c_int32), ('lfnst_set', ctypes.c_int32), ('lfnst_transpose', ctypes.c_int32),
@@ -115,6 +123,9 @@ BI_BEST_DT = np.dtype([('int_hor', '<i4'), ('int_ver', '<i4'), ('int_best', '<u8
                        ('qter_ver', '<i2'), ('mv_hor', '<i4'), ('mv_ver', '<i4'), ('bits', '<u4'), ('pad', '<u4'), ('cost', '<u8')])
 BI_PAR = vvb_bi_par
 assert BI_PU_DT.itemsize == 36 and BI_BEST_DT.itemsize == 56 and ctypes.sizeof(vvb_bi_par) == 56
+AMVP_DT = np.dtype([('cand_hor', '<i4', (2,)), ('cand_ver', '<i4', (2,)), ('num_cand', '<i4'), ('mvp_idx', '<i4')])
+AMVR_BEST_DT = np.dtype([('mv_hor', '<i4'), ('mv_ver', '<i4'), ('mvp_idx', '<i4'), ('bits', '<u4'), ('dist', '<u8'), ('cost', '<u8')])
+assert AMVP_DT.itemsize == 24 and AMVR_BEST_DT.itemsize == 32 and ctypes.sizeof(vvb_amvr_par) == 40
 assert CAND_DT.itemsize == 32 and BLOCK_DT.itemsize == 24 and BEST_DT.itemsize == 16 and MCTF_DT.itemsize == 20
 
 # every symbol include/vvenc_b200.h declares: name -> (restype, argtypes)
@@ -202,6 +213,10 @@ SYMBOLS = {
     'vvb_frac_search_dev': (c_i, [c_p, c_i, c_i, c_p, c_p, c_i, c_i, c_i, ctypes.POINTER(vvb_frac_par), c_p]),
     'vvb_bipred_search': (c_i, [c_p, c_i, c_i, c_p, c_i, c_i, c_i, ctypes.POINTER(vvb_bi_par), c_p, c_i, c_p, c_p]),
     'vvb_bipred_search_dev': (c_i, [c_p, c_i, c_i, c_p, c_i, c_i, c_i, ctypes.POINTER(vvb_bi_par), c_p, c_i, c_p, c_p]),
+    'vvb_amvr_refine': (c_i, [c_p, c_i, c_i, c_p, c_p, c_p, c_p, c_i, c_i, c_i, ctypes.POINTER(vvb_amvr_par), c_p]),
+    'vvb_amvr_refine_dev': (c_i, [c_p, c_i, c_i, c_p, c_p, c_p, c_p, c_i, c_i, c_i, ctypes.POINTER(vvb_amvr_par), c_p]),
+    'vvb_bipred_amvr_search': (c_i, [c_p, c_i, c_i, c_p, c_p, c_i, c_i, c_i, ctypes.POINTER(vvb_bi_par), c_p, c_p, c_i, c_p, c_p, c_p]),
+    'vvb_bipred_amvr_search_dev': (c_i, [c_p, c_i, c_i, c_p, c_p, c_i, c_i, c_i, ctypes.POINTER(vvb_bi_par), c_p, c_p, c_i, c_p, c_p, c_p]),
     'vvb_mctf_apply': (c_i, [c_p, c_i, ctypes.POINTER(vvb_mctf_apply_par), c_p, c_p, c_i]),
     'vvb_mctf_apply_dev': (c_i, [c_p, c_i, ctypes.POINTER(vvb_mctf_apply_par), c_p, c_p, c_i]),
     'vvb_mctf_calc_var': (c_i, [c_p, c_i, c_p, c_i, c_p]),

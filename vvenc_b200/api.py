@@ -303,6 +303,40 @@ class CostEngine:
                                              _p(cands) if len(cands) else None, len(cands), _p(pred), _p(out)))
         return out
 
+    @staticmethod
+    def amvr_par(lambda_, dfunc, imv, mvp_bits, pic_w, pic_h, ctu_size, ifp_lines=0):
+        """settings of amvr_refine: imv 1 (IMV_FPEL) or 2 (IMV_4PEL); mvp_bits = (m_auiMVPIdxCost[0][2], m_auiMVPIdxCost[1][2])"""
+        return L.vvb_amvr_par(float(lambda_), dfunc, imv, (ctypes.c_uint32 * 2)(*[int(b) & 0xffffffff for b in mvp_bits]), pic_w, pic_h, ctu_size, ifp_lines)
+
+    def amvr_refine(self, org_plane, ref_plane, pus, int_mv, amvp, bits, w, h, par):
+        """InterSearch::xPatternSearchIntRefine (uni-prediction, fWeight 1.0) for every PU of one shape.  pus: TZ_PU_DT (x, y, pred_hor, pred_ver used);
+        int_mv: TZ_BEST_DT (mv_hor, mv_ver used), e.g. what tz_search returned with imv_shift 2 or 4; amvp: AMVP_DT; bits: uint32 ruiBits per PU.
+        Returns an AMVR_BEST_DT array (final rcMv in 1/16 pel, riMVPIdx, ruiBits, uiBestDist, ruiCost)."""
+        pus = np.ascontiguousarray(pus, dtype=L.TZ_PU_DT)
+        int_mv = np.ascontiguousarray(int_mv, dtype=L.TZ_BEST_DT)
+        amvp = np.ascontiguousarray(amvp, dtype=L.AMVP_DT)
+        bits = np.ascontiguousarray(bits, dtype=np.uint32)
+        assert len(pus) == len(int_mv) == len(amvp) == len(bits)
+        out = np.zeros(len(pus), dtype=L.AMVR_BEST_DT)
+        self._chk(self.lib.vvb_amvr_refine(self.h, org_plane, ref_plane, _p(pus), _p(int_mv), _p(amvp), _p(bits), len(pus), w, h, ctypes.byref(par), _p(out)))
+        return out
+
+    def bipred_amvr_search(self, org_plane, ref_plane, pus, amvp, w, h, par, mvp_bits, pred, cands=None):
+        """The bi-predictive branch of InterSearch::xMotionEstimation for cu.imv 1 and 2 (par.imv) for every PU of one shape: the integer stage of
+        bipred_search, then xPatternSearchIntRefine on the target with the BCW weight.  pus: BI_PU_DT; amvp: AMVP_DT; mvp_bits as amvr_par's; pred: int16
+        [n][h][w].  Returns (TZ_BEST_DT integer stage, AMVR_BEST_DT result)."""
+        pus = np.ascontiguousarray(pus, dtype=L.BI_PU_DT)
+        amvp = np.ascontiguousarray(amvp, dtype=L.AMVP_DT)
+        pred = np.ascontiguousarray(pred, dtype=np.int16)
+        assert pred.shape == (len(pus), h, w) and len(amvp) == len(pus)
+        cands = np.zeros((0, 2), dtype=np.int32) if cands is None else np.ascontiguousarray(cands, dtype=np.int32).reshape(-1, 2)
+        mb = np.array([int(b) & 0xffffffff for b in mvp_bits], dtype=np.uint32)
+        int_out = np.zeros(len(pus), dtype=L.TZ_BEST_DT)
+        out = np.zeros(len(pus), dtype=L.AMVR_BEST_DT)
+        self._chk(self.lib.vvb_bipred_amvr_search(self.h, org_plane, ref_plane, _p(pus), _p(amvp), len(pus), w, h, ctypes.byref(par), _p(mb),
+                                                  _p(cands) if len(cands) else None, len(cands), _p(pred), _p(int_out), _p(out)))
+        return int_out, out
+
     # ---- dependent quantisation
     def set_depquant_engine(self, engine):
         self._chk(self.lib.vvb_set_depquant_engine(self.h, int(engine)))

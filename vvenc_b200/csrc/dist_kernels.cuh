@@ -67,7 +67,7 @@ __device__ __forceinline__ uint32_t group_sad( const int16_t* __restrict__ org, 
 }
 
 // SSE (CommonLib/RdCost.cpp:651-1000): 64-bit exact
-template<int G>
+template<int G, bool ORG_SMEM = false>
 __device__ __forceinline__ unsigned long long group_sse( const int16_t* __restrict__ org, int so, const int16_t* __restrict__ cur, int sc,
                                                          int w, int h, int lg )
 {
@@ -79,7 +79,7 @@ __device__ __forceinline__ unsigned long long group_sse( const int16_t* __restri
     for( int i = lg; i < total; i += G )
     {
       const int y = i >> lc, c = i & ( cpr - 1 );
-      const uint32_t a = __ldg( reinterpret_cast<const uint32_t*>( org + (size_t) y * so ) + c );
+      const uint32_t a = org_load<ORG_SMEM>( reinterpret_cast<const uint32_t*>( org + (size_t) y * so ) + c );
       const uint32_t b = __ldg( reinterpret_cast<const uint32_t*>( cur + (size_t) y * sc ) + c );
       const int d0 = lo16( a ) - lo16( b ), d1 = hi16( a ) - hi16( b );
       acc += (unsigned long long)( (long long) d0 * d0 ) + (unsigned long long)( (long long) d1 * d1 );
@@ -91,7 +91,7 @@ __device__ __forceinline__ unsigned long long group_sse( const int16_t* __restri
     for( int i = lg; i < total; i += G )
     {
       const int y = i >> lw, x = i & ( w - 1 );
-      const int d = (int) __ldg( org + (size_t) y * so + x ) - (int) __ldg( cur + (size_t) y * sc + x );
+      const int d = (int) org_load<ORG_SMEM>( org + (size_t) y * so + x ) - (int) __ldg( cur + (size_t) y * sc + x );
       acc += (unsigned long long)( (long long) d * d );
     }
   }
@@ -136,15 +136,15 @@ template<int TW> __device__ __forceinline__ void wht_regs( int (&d)[TW] )
   }
 }
 
-// loads TW differences org-cur of one tile row; also accumulates sum|d| for HAD_2SAD
-template<int TW> __device__ __forceinline__ void load_diff_row( const int16_t* __restrict__ o, const int16_t* __restrict__ c, int (&d)[TW], int& sadAcc )
+// loads TW differences org-cur of one tile row; also accumulates sum|d| for HAD_2SAD.  ORG_SMEM: org is read from shared memory (org_load)
+template<int TW, bool ORG_SMEM = false> __device__ __forceinline__ void load_diff_row( const int16_t* __restrict__ o, const int16_t* __restrict__ c, int (&d)[TW], int& sadAcc )
 {
   if( TW >= 8 && ( ( (uintptr_t) o | (uintptr_t) c ) & 15 ) == 0 )
   {
 #pragma unroll
     for( int v = 0; v < TW / 8; v++ )
     {
-      const uint4 a = __ldg( reinterpret_cast<const uint4*>( o ) + v ), b = __ldg( reinterpret_cast<const uint4*>( c ) + v );
+      const uint4 a = org_load<ORG_SMEM>( reinterpret_cast<const uint4*>( o ) + v ), b = __ldg( reinterpret_cast<const uint4*>( c ) + v );
       d[8*v+0] = lo16( a.x ) - lo16( b.x ); d[8*v+1] = hi16( a.x ) - hi16( b.x );
       d[8*v+2] = lo16( a.y ) - lo16( b.y ); d[8*v+3] = hi16( a.y ) - hi16( b.y );
       d[8*v+4] = lo16( a.z ) - lo16( b.z ); d[8*v+5] = hi16( a.z ) - hi16( b.z );
@@ -156,14 +156,14 @@ template<int TW> __device__ __forceinline__ void load_diff_row( const int16_t* _
 #pragma unroll
     for( int v = 0; v < TW / 2; v++ )
     {
-      const uint32_t a = __ldg( reinterpret_cast<const uint32_t*>( o ) + v ), b = __ldg( reinterpret_cast<const uint32_t*>( c ) + v );
+      const uint32_t a = org_load<ORG_SMEM>( reinterpret_cast<const uint32_t*>( o ) + v ), b = __ldg( reinterpret_cast<const uint32_t*>( c ) + v );
       d[2*v] = lo16( a ) - lo16( b ); d[2*v+1] = hi16( a ) - hi16( b );
     }
   }
   else
   {
 #pragma unroll
-    for( int x = 0; x < TW; x++ ) d[x] = (int) __ldg( o + x ) - (int) __ldg( c + x );
+    for( int x = 0; x < TW; x++ ) d[x] = (int) org_load<ORG_SMEM>( o + x ) - (int) __ldg( c + x );
   }
 #pragma unroll
   for( int x = 0; x < TW; x++ ) sadAcc += abs( d[x] );
@@ -199,7 +199,7 @@ template<int TW> __device__ __forceinline__ uint32_t had_tile_lanes( int (&d)[TW
   return (uint32_t)(int)( __ddiv_rn( (double)(int) s, sqrt( 4.0 * 8 ) ) * 2.0 );                       // 8x4 / 4x8: :1682,:1763
 }
 
-template<int G, int TW>
+template<int G, int TW, bool ORG_SMEM = false>
 __device__ __forceinline__ void group_had_tw( const int16_t* __restrict__ org, int so, const int16_t* __restrict__ cur, int sc, int w, int h,
                                               const HadShape& s, int lg, uint32_t& hadSum, uint32_t& sadSum )
 {
@@ -227,14 +227,14 @@ __device__ __forceinline__ void group_had_tw( const int16_t* __restrict__ org, i
 #pragma unroll
         for( int x = 0; x < TW; x++ )
         {
-          const int ov = ( (int) __ldg( o + 2*x ) + __ldg( o + 2*x + 1 ) + __ldg( o + so + 2*x ) + __ldg( o + so + 2*x + 1 ) + 2 ) >> 2;
+          const int ov = ( (int) org_load<ORG_SMEM>( o + 2*x ) + org_load<ORG_SMEM>( o + 2*x + 1 ) + org_load<ORG_SMEM>( o + so + 2*x ) + org_load<ORG_SMEM>( o + so + 2*x + 1 ) + 2 ) >> 2;
           const int cv = ( (int) __ldg( c + 2*x ) + __ldg( c + 2*x + 1 ) + __ldg( c + sc + 2*x ) + __ldg( c + sc + 2*x + 1 ) + 2 ) >> 2;
           d[x] = ov - cv;
         }
       }
       else
       {
-        load_diff_row<TW>( org + (size_t)( ty * s.th + row ) * so + tx * TW, cur + (size_t)( ty * s.th + row ) * sc + tx * TW, d, sadAcc );
+        load_diff_row<TW, ORG_SMEM>( org + (size_t)( ty * s.th + row ) * so + tx * TW, cur + (size_t)( ty * s.th + row ) * sc + tx * TW, d, sadAcc );
       }
     }
     const uint32_t v = had_tile_lanes<TW>( d, th, row, active, gmask<G>() );
@@ -244,21 +244,21 @@ __device__ __forceinline__ void group_had_tw( const int16_t* __restrict__ org, i
   sadSum = group_sum_u32<G>( (uint32_t) sadAcc );
 }
 
-// family dispatch for one candidate evaluated by a G-lane group; returns the cost in every lane of the group
-template<int G>
+// family dispatch for one candidate evaluated by a G-lane group; returns the cost in every lane of the group.  ORG_SMEM: org is a block staged in shared memory
+template<int G, bool ORG_SMEM = false>
 __device__ __forceinline__ unsigned long long group_dist( int fam, const int16_t* __restrict__ org, int so, const int16_t* __restrict__ cur, int sc,
                                                           int w, int h, int subShift, int lg )
 {
-  if( fam == FAM_SAD ) return group_sad<G>( org, so, cur, sc, w, h, subShift, lg );
-  if( fam == FAM_SSE ) return group_sse<G>( org, so, cur, sc, w, h, lg );
+  if( fam == FAM_SAD ) return group_sad<G, ORG_SMEM>( org, so, cur, sc, w, h, subShift, lg );
+  if( fam == FAM_SSE ) return group_sse<G, ORG_SMEM>( org, so, cur, sc, w, h, lg );
   HadShape s;
   if( !had_shape( w, h, fam == FAM_HAD_FAST, s ) ) return ~0ull;
   uint32_t had = 0, sad = 0;
   const int tw = s.fast16 ? 8 : s.tw;
-  if( G >= 16 && tw == 16 )     group_had_tw<G, 16>( org, so, cur, sc, w, h, s, lg, had, sad );
-  else if( tw == 8 )            group_had_tw<G, 8 >( org, so, cur, sc, w, h, s, lg, had, sad );
-  else if( tw == 4 )            group_had_tw<G, 4 >( org, so, cur, sc, w, h, s, lg, had, sad );
-  else if( tw == 2 )            group_had_tw<G, 2 >( org, so, cur, sc, w, h, s, lg, had, sad );
+  if( G >= 16 && tw == 16 )     group_had_tw<G, 16, ORG_SMEM>( org, so, cur, sc, w, h, s, lg, had, sad );
+  else if( tw == 8 )            group_had_tw<G, 8,  ORG_SMEM>( org, so, cur, sc, w, h, s, lg, had, sad );
+  else if( tw == 4 )            group_had_tw<G, 4,  ORG_SMEM>( org, so, cur, sc, w, h, s, lg, had, sad );
+  else if( tw == 2 )            group_had_tw<G, 2,  ORG_SMEM>( org, so, cur, sc, w, h, s, lg, had, sad );
   if( fam == FAM_HAD_2SAD ) return had < 2u * sad ? had : 2u * sad;       // RdCost.cpp:1815
   return had;
 }
